@@ -2,7 +2,7 @@
 """bench.py -- headline benchmark of libdeflate_b200 (contract in the task brief, section 4).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
-                    [--workload roundtrip|decompress] [--chunks C] [--chunk-size B]
+                    [--workload roundtrip|decompress] [--chunks C] [--chunk-size B] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): a batch of 65 536 x 64 KiB synthetic text-like
 chunks PER GPU (weak scaling; configs[4] is the same shape at 8 GPUs), gzip level 6
@@ -17,6 +17,8 @@ value  = kernel-path throughput, inputs resident in HBM, CUDA events on the laun
 e2e    = same metric through libdeflate_b200_*_batch_host with pinned HOST buffers
          (H2D of the inputs and D2H of the results inside the timed region).
 roofline / cpu_baseline: see DESIGN.md section "Measurement".
+--dump-outputs DIR: what the last timed step returned (see dump_outputs), so that two builds can be
+         compared output for output; the inputs are the same from run to run.
 """
 import argparse
 import ctypes
@@ -24,6 +26,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -45,7 +48,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -104,9 +107,11 @@ def dist_env():
 
 
 def load_synth():
-    if not os.path.exists(SYNTH_SO):
-        subprocess.check_call(["gcc", "-O2", "-fPIC", "-shared", "-pthread", "-o", SYNTH_SO, os.path.join(ROOT, "bench", "synth.c"), "-lm"])
-    l = ctypes.CDLL(SYNTH_SO)
+    so = SYNTH_SO
+    if not os.path.exists(so):      # not built in the tree: build it outside (the tree may be read-only)
+        so = os.path.join(tempfile.mkdtemp(prefix="ldb_synth_"), "libsynth.so")
+        subprocess.check_call(["gcc", "-O2", "-fPIC", "-shared", "-pthread", "-o", so, os.path.join(ROOT, "bench", "synth.c"), "-lm"])
+    l = ctypes.CDLL(so)
     l.synth_fill.restype = None
     l.synth_fill.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_size_t, ctypes.c_int, ctypes.c_int]
     return l
@@ -182,7 +187,7 @@ def run_reference(args):
         return
     cpub = load_cpub()
     if cpub is None:
-        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/libcpubench.so not built (needs /root/reference at build time)"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/libcpubench.so not built (needs LIBDEFLATE_REF=<reference source tree> at build time)"}))
         return
     synth = load_synth()
     threads = host_threads()
@@ -250,7 +255,7 @@ def workload_config(args, n_override=None):
         w = "batch of %d x %d B synthetic text chunks per GPU, gzip level %d compress+decompress" % (n, args.chunk_size, LEVEL)
     return {"workload": w, "chunks_per_gpu": n, "chunk_bytes": args.chunk_size, "level": LEVEL,
             "format": "raw" if args.workload == "decompress" else "gzip",
-            "l2_policy": "inputs (%.1f GiB per GPU) are far larger than the 126 MB L2; no explicit flush" % (n * args.chunk_size / 2.0**30),
+            "l2_policy": "inputs (%.1f GiB per GPU) are far larger than the 50 MB L2; no explicit flush" % (n * args.chunk_size / 2.0**30),
             "parallelism": "independent chunk shards per GPU, no data-path collective (the single-origin NCCL scatter/gather run of the same batch is reported under single_origin when N > 1)"}
 
 
@@ -342,6 +347,41 @@ def roofline_entry(kernels, ms_total, launches, alg_bytes, traffic_db, traffic_k
             "avg_launch_ms": round(per * 1e3, 4), "algorithmic_bytes_per_launch": int(alg_bytes)}
 
 
+DUMP_BUDGET = 48 << 20      # bytes of sampled chunks (float32: 4 bytes per byte); the whole-batch arrays come on top
+DUMP_CHUNKS_MAX = 64
+
+
+def dump_outputs(out_dir, ctx, l, n, chunk, cstride, d_comp, d_csz, d_out, d_aout, d_res, roundtrip):
+    """What the caller of the timed calls received in the last step, as float64 / float32 .npy files: per-chunk
+    results, output sizes and (round trip) compressed sizes of the whole batch (24 bytes per chunk); the compressed
+    streams (zero-padded rows) and decompressed bytes of up to DUMP_CHUNKS_MAX chunks picked by a fixed seed, as many
+    as fit DUMP_BUDGET (64 x 64 KiB chunks: 35 MB in all; 5 x 1 MiB chunks: 42 MB)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    res = np.empty(n, dtype=np.int32)
+    aout = np.empty(n, dtype=np.uint64)
+    csz = np.empty(n, dtype=np.uint64)
+    ctx._check(l.libdeflate_b200_memcpy_d2h(ctx.h, res.ctypes.data, d_res, 4 * n), "d2h")
+    ctx._check(l.libdeflate_b200_memcpy_d2h(ctx.h, aout.ctypes.data, d_aout, 8 * n), "d2h")
+    ctx._check(l.libdeflate_b200_memcpy_d2h(ctx.h, csz.ctypes.data, d_csz, 8 * n), "d2h")
+    ctx.sync()
+    k = max(1, min(n, DUMP_CHUNKS_MAX, DUMP_BUDGET // (4 * (chunk + cstride))))
+    idx = np.sort(np.random.default_rng(0).choice(n, size=k, replace=False))
+    comp = np.zeros((len(idx), cstride), dtype=np.uint8)
+    plain = np.empty((len(idx), chunk), dtype=np.uint8)
+    for row, i in enumerate(idx.tolist()):
+        ctx._check(l.libdeflate_b200_memcpy_d2h(ctx.h, comp[row].ctypes.data, d_comp.slab + i * cstride, int(csz[i])), "d2h")
+        ctx._check(l.libdeflate_b200_memcpy_d2h(ctx.h, plain[row].ctypes.data, d_out.slab + i * chunk, chunk), "d2h")
+    ctx.sync()
+    arrays = {"results": res.astype(np.float64), "actual_out_sizes": aout.astype(np.float64),
+              "sample_chunk_index": idx.astype(np.float64), "decompressed_sample": plain.astype(np.float32)}
+    if roundtrip:
+        arrays["compressed_sizes"] = csz.astype(np.float64)
+        arrays["compressed_sample"] = comp.astype(np.float32)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def run_b200(args):
     import numpy as np
     import libdeflate_b200 as ldb
@@ -400,7 +440,7 @@ def run_b200(args):
 
     def load_reference_streams():
         """the reference's own L6 raw streams for the same chunks (SURVEY.md section 8d) -> d_comp / d_csz"""
-        assert cpub is not None, "the decompress workload needs oracle/_ref (prebuilt from /root/reference)"
+        assert cpub is not None, "the decompress workload needs oracle/_ref (built when LIBDEFLATE_REF names the reference sources)"
         comp = (ctypes.c_uint8 * (cstride * n))()
         sizes = (ctypes.c_size_t * n)()
         fails = ctypes.c_int(0)
@@ -454,6 +494,8 @@ def run_b200(args):
     clocks = ClockSampler(local) if rank == 0 else None
     ms, ktime, launches, clk = timed_steps(ctx, l, step, args.steps, args.warmup, barrier, clocks)
     ms_max = max(allmax(ms), 1e-9)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ctx, l, n, chunk, cstride, d_comp, d_csz, d_out, d_aout, d_res, args.workload == "roundtrip")
 
     # ---- verification (outside the timed region) ----------------------------------------
     c2 = check_outputs("main workload")
@@ -614,14 +656,19 @@ def run_b200(args):
         for p_ in (d_csz, d_aout, d_res):
             l.libdeflate_b200_device_free(ctx.h, p_)
         dev = torch.device("cuda", local)
-        n_total = n * world
+        # the root holds the whole batch three times (input, packed streams, output) beside its own shard's buffers
+        # and the token scratch: on an 80 GB GPU that caps the single-origin batch below N x the pre-sharded one at N >= 4.
+        # The cap is an estimate from those sizes; it has not yet been run on a multi-GPU H100 machine.
+        cap = (torch.cuda.get_device_properties(dev).total_memory - (16 << 30)) // 5 // chunk
+        n_total = min(n * world, cap)
         rt = shard.OriginRoundTrip(ctx, dist, dev, n_total, chunk, fmt, LEVEL, stages=8)
         root_in = None
         if rank == 0:
             root_in = torch.empty(n_total * chunk, dtype=torch.uint8, device=dev)
-            for r in range(world):        # the batch of the pre-sharded run, rank by rank, through the one pinned buffer
-                synth.synth_fill(pin_in, chunk, r * n, n, getattr(args, "data_class", 0), threads)
-                ctx._check(l.libdeflate_b200_memcpy_h2d(ctx.h, root_in.data_ptr() + r * n * chunk, pin_in, n * chunk), "h2d")
+            for lo in range(0, n_total, n):        # the first chunks of the pre-sharded run's batch, through the one pinned buffer
+                k = min(n, n_total - lo)
+                synth.synth_fill(pin_in, chunk, lo, k, getattr(args, "data_class", 0), threads)
+                ctx._check(l.libdeflate_b200_memcpy_h2d(ctx.h, root_in.data_ptr() + lo * chunk, pin_in, k * chunk), "h2d")
                 ctx.sync()
         so_steps = max(1, min(args.steps, 2))
         info = rt.step(root_in)           # warm-up (NCCL channels, scratch)
@@ -741,7 +788,7 @@ def run_e2e(args, ctx, l, ldb, pin_in, n, chunk, fmt, cstride, barrier, allmax, 
     if args.workload == "roundtrip" and ne >= int(os.environ.get("LDB_E2E_GROUP_MIN", "4096")) and getattr(args, "overlap", False):
         # The same two calls with the batch going through in GROUPS: one host thread compresses group g + 1 (own
         # context = own stream) while a second one decompresses group g, to hide the decompress call's PCIe time
-        # behind the deflate kernel of the next group.  Measured: it does not pay (profiles/r02_e2e_overlap.md).
+        # behind the deflate kernel of the next group.
         import threading
         groups = 4
         ng = ne // groups
@@ -830,9 +877,9 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the short legs of the other BASELINE configs (decompress-only, checksums, level 12)")
     ap.add_argument("--no-l12", action="store_true", help="skip the level-12 4096 x 1 MiB leg")
-    ap.add_argument("--overlap", action="store_true", help="e2e: also measure the two-host-thread form (compress of group g+1 over decompress of group g); "
-                    "measured slower than the plain form (9.3 vs 10.06 GB/s, profiles/r02_e2e_overlap.md), hence off by default")
+    ap.add_argument("--overlap", action="store_true", help="e2e: also measure the two-host-thread form (compress of group g+1 over decompress of group g)")
     ap.add_argument("--no-origin", action="store_true", help="N > 1: skip the single-origin (NCCL scatter/gather) leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned to DIR/<name>.npy")
     args = ap.parse_args()
     LEVEL = args.level
     if args.warmup < 3:

@@ -7,7 +7,7 @@
  * written against ebiggers/libdeflate compiles and links against
  * libdeflate_b200.so unchanged.  The implementation behind every symbol is a
  * thin host shim (libdeflate_b200/csrc/shim.cu) that launches hand-written
- * sm_100a CUDA kernels; there is no CPU fallback.  The throughput API that
+ * sm_90a CUDA kernels; there is no CPU fallback.  The throughput API that
  * processes a batch of independent chunks per launch is the additive extension
  * declared in libdeflate_b200.h.
  *

@@ -3,7 +3,7 @@
  *
  * The reference processes one buffer per call and leaves the "batch of
  * independent chunks" loop to its callers (ref: programs/benchmark.c:443-509,
- * README.md:122-135).  On a B200 that loop is the grid: every entry point here
+ * README.md:122-135).  On an H100 that loop is the grid: every entry point here
  * takes N independent chunks and runs them in ONE kernel launch sequence on the
  * context's CUDA stream.  Per-chunk semantics (verdicts, byte counts, bounds)
  * are exactly those of the single-buffer call in libdeflate.h that each entry

@@ -1,9 +1,9 @@
-"""libdeflate_b200 -- B200-native batched DEFLATE / zlib / gzip / CRC-32 / Adler-32.
+"""libdeflate_b200 -- H100-native batched DEFLATE / zlib / gzip / CRC-32 / Adler-32.
 
 Python here is plumbing only: a ctypes mirror of the C ABI declared in
 ``include/libdeflate.h`` (the 21 reference symbols, ref: libdeflate.h:59-365) and
 ``include/libdeflate_b200.h`` (the additive batch extension).  All compute happens in
-hand-written sm_100a CUDA kernels inside ``libdeflate_b200.so``; there is no CPU
+hand-written sm_90a CUDA kernels inside ``libdeflate_b200.so``; there is no CPU
 fallback -- loading fails loudly if the library is not built, and every compute call
 fails loudly if no CUDA device is present.
 

@@ -1,4 +1,4 @@
-"""Build driver for libdeflate_b200.so (the C-ABI library with the sm_100a kernels).
+"""Build driver for libdeflate_b200.so (the C-ABI library with the sm_90a kernels).
 
     python -m libdeflate_b200.build          # nvcc build, in-tree
     python -m libdeflate_b200.build --emu    # g++ build against tests/emu (CPU logic tests only)
@@ -19,8 +19,9 @@ LIB = os.path.join(HERE, "libdeflate_b200.so")
 EMU_DIR = os.path.join(ROOT, "tests", "emu")
 EMU_LIB = os.path.join(EMU_DIR, "_build", "libdeflate_b200_emu.so")
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]     # H100 (Hopper)
+NVCC_FLAGS = ARCH + [
+    "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "--use_fast_math", "-Xptxas", "-v",
 ]
 
@@ -39,7 +40,7 @@ def _deps():
 
 
 def build(verbose=False, force=False):
-    """Compile every .cu for sm_100a and link libdeflate_b200.so in-tree."""
+    """Compile every .cu for sm_90a and link libdeflate_b200.so in-tree."""
     if not force and not _newer(LIB, _deps() + [os.path.abspath(__file__)]):
         return LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -62,7 +63,7 @@ def build(verbose=False, force=False):
         f.write("\n".join(logs))
     if verbose:
         print("\n".join(logs))
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-Xlinker", "--exclude-libs,ALL"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-lcudart_static", "-Xlinker", "--exclude-libs,ALL"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,4 +1,4 @@
-// checksum_kernels.cu -- batched CRC-32 and Adler-32 for sm_100a.
+// checksum_kernels.cu -- batched CRC-32 and Adler-32 for sm_90a.
 //
 // What it computes (bit-exact with the reference):
 //   crc32 : libdeflate_crc32()  ref: lib/crc32.c:256-262 (gzip CRC-32, reflected
@@ -7,7 +7,7 @@
 //   adler32: libdeflate_adler32() ref: lib/adler32.c:156-162 (s1 = 1 + sum b,
 //           s2 = sum of running s1, both mod 65521).
 //
-// B200 mapping (not a port of the PCLMUL / VNNI paths, there is no carry-less
+// H100 mapping (not a port of the PCLMUL / VNNI paths, there is no carry-less
 // multiply on the GPU):
 //   * one warp per chunk, grid-stride over the batch; every global load is a
 //     coalesced 16-byte vector load (32 lanes x 16 B = one 512-B row per step),

@@ -1,4 +1,4 @@
-// deflate_kernel.cu -- batched DEFLATE / zlib / gzip compression for sm_100a.
+// deflate_kernel.cu -- batched DEFLATE / zlib / gzip compression for sm_90a.
 //
 // What it computes: for every chunk i, a valid stream of the requested format that
 // inflates to in[i] and fits libdeflate_*_compress_bound(); out_nbytes[i] = bytes

@@ -1,4 +1,4 @@
-// deflate_lz_kernel.cuh -- LZ77 match finding + parsing + Huffman block encoding, sm_100a.
+// deflate_lz_kernel.cuh -- LZ77 match finding + parsing + Huffman block encoding, sm_90a.
 // Included by deflate_kernel.cu.
 //
 // Reference behaviour covered (what, not how):
@@ -9,7 +9,7 @@
 // The output is a valid DEFLATE stream with a ratio close to the reference's at the
 // same level, never the reference's bytes (libdeflate.h:76-83 makes no such promise).
 //
-// B200 mapping: one persistent CTA (1024 threads) per chunk; everything a chunk needs
+// H100 mapping: one persistent CTA (1024 threads) per chunk; everything a chunk needs
 // lives in shared memory (~224 KiB):
 //   * a 64 KiB ring of the input (the sliding window), filled 16 KiB at a time by the
 //     TMA bulk-copy engine (cp.async.bulk + mbarrier) -- the window never touches

@@ -1,4 +1,4 @@
-// inflate_kernel.cu -- batched DEFLATE / zlib / gzip decompression for sm_100a.
+// inflate_kernel.cu -- batched DEFLATE / zlib / gzip decompression for sm_90a.
 //
 // What it computes: for every chunk i of the batch, exactly what
 //   libdeflate_{deflate,zlib,gzip}_decompress_ex()   (ref: lib/decompress_template.h:44-772,
@@ -14,12 +14,12 @@
 //       chunk's scratch slot, 4-byte {literal run, length, offset} records from its back, format
 //       in ldb_common.cuh).  Every verdict, actual_in and actual_out are decided here: the
 //       decoder tracks the output position, so "offset > bytes produced" and "no room" need no
-//       output bytes.  No LZ77 window is touched -- with ~71 K streams in flight the windows
-//       (4.6 GB) can live nowhere but DRAM, which is what bound the one-kernel design of round 1.
+//       output bytes.  No LZ77 window is touched -- with ~68 K streams in flight the windows
+//       (2.2 GB) can live nowhere but DRAM, which is what bounds a one-kernel design.
 //   ldb_inflate_resolve_kernel (inflate_resolve.cu) -- one CTA per chunk turns the tokens into
 //       bytes inside a shared-memory window.
 //
-// B200 mapping of the decode kernel -- "one lane per stream", because Huffman decoding is a
+// H100 mapping of the decode kernel -- "one lane per stream", because Huffman decoding is a
 // bit-serial dependency chain and only issue slots spent on *different* streams add up:
 //   * a warp decodes 32 independent chunks at once, one per lane; a lane that
 //     finishes its chunk pulls the next chunk index from a global counter, so
@@ -27,11 +27,11 @@
 //   * each lane's decode tables live in shared memory, lane-interleaved
 //     (entry i of lane t sits in bank t), so the 32 data-dependent lookups of a
 //     warp instruction are bank-conflict free by construction;
-//   * tables are compact 16-bit entries: 7-bit main litlen table + 32 subtable
-//     entries, 5-bit main offset table + 32 subtable entries = 448 B per lane,
-//     14 KiB per warp, 14 single-warp CTAs per SM (occupancy is what this
-//     latency-bound kernel lives on: 4 -> 7 -> 14 warps/SM measured 31 -> 65 ->
-//     141 GB/s); subtable entries beyond the shared-memory capacity live in a
+//   * tables are compact 16-bit entries: 7-bit main litlen table + 24 subtable
+//     entries, 5-bit main offset table + 32 subtable entries = 432 B per lane,
+//     14 KiB per warp, 16 warps per SM (occupancy is what this latency-bound
+//     kernel lives on, and 132 SMs x 16 warps x 32 lanes hold a batch of 65536
+//     chunks in one wave); subtable entries beyond the shared-memory capacity live in a
 //     per-lane global scratch (L1/L2 resident);
 //   * block headers are parsed by the owning lane, then the WARP builds that
 //     lane's tables cooperatively (ballot/match_any ranking, strided fills);
@@ -64,7 +64,7 @@
 #endif
 #define INF_LMAIN     (1 << INF_LB)
 #ifndef INF_LSUB_SM
-#define INF_LSUB_SM   32		// litlen subtable entries kept in shared memory
+#define INF_LSUB_SM   24		// litlen subtable entries kept in shared memory (24, not 32: 16 warps fit an SM)
 #endif
 #define INF_LSUB_CAP  2048		// total litlen subtable capacity (rest in global scratch)
 #ifndef INF_OB
@@ -117,9 +117,9 @@
 #ifndef INF_WQ2
 #define INF_WQ2 0		// 1: two lookahead words per lane, one copy group per step (profiles/r02_inflate_d.md, call P)
 #endif
-#define INF_SM_BYTES   (INF_SM_WQ + 128 + 128 * INF_WQ2)		// per warp: 14720 with the default geometry
+#define INF_SM_BYTES   (INF_SM_WQ + 128 + 128 * INF_WQ2)		// per warp: 14208 with the default geometry
 #ifndef INF_WPC
-#define INF_WPC        5		// independent warps per CTA
+#define INF_WPC        8		// independent warps per CTA
 #endif
 
 static_assert(INF_O_ENTRIES >= 64, "the offset region doubles as the 128-byte precode table scratch");
@@ -319,8 +319,8 @@ __device__ __forceinline__ void inf_put_match(inf_lane &s, u32 length, u32 offse
 
 // ---- warp-wide copy of a stored block into the literal stream -----------------------------------
 // dst/src/len are warp-uniform, alignments arbitrary.  16-byte rows of the destination are built from
-// five aligned source words and funnel shifts, two rows per lane in flight (a byte-per-lane loop paid one
-// global round trip per 32 bytes: 17 ms for 16384 incompressible 64 KiB chunks); rows are only taken
+// five aligned source words and funnel shifts, two rows per lane in flight (a byte-per-lane loop pays one
+// global round trip per 32 bytes); rows are only taken
 // where all five words lie inside the block, the ragged ends go byte by byte.
 __device__ __forceinline__ void inf_warp_copy(u8 *dst, const u8 *src, u32 len, u32 lane)
 {
@@ -895,9 +895,9 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 // ---- the decode kernel --------------------------------------------------------------
 // The warps of a CTA are independent (each has its own tables and never syncs with the others);
 // INF_WPC of them share a CTA only because shared memory is reserved per CTA (1 KiB each), and
-// 3 CTAs x 5 warps fit where 15 single-warp CTAs would not.
+// 2 CTAs x 8 warps fit where 16 single-warp CTAs would not.
 #ifndef INF_MIN_CTAS
-#define INF_MIN_CTAS 3		// CTAs per SM the register allocation must allow
+#define INF_MIN_CTAS 2		// CTAs per SM the register allocation must allow
 #endif
 __global__ void __launch_bounds__(32 * INF_WPC, INF_MIN_CTAS)
 ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)

@@ -1,4 +1,4 @@
-// inflate_resolve.cu -- second half of batched DEFLATE decompression for sm_100a: the LZ77
+// inflate_resolve.cu -- second half of batched DEFLATE decompression for sm_90a: the LZ77
 // side.  (First half: inflate_kernel.cu, which turns every stream into tokens.)
 //
 // What it computes: for every chunk whose stream decoded, the bytes the reference's decode
@@ -6,16 +6,15 @@
 // forward byte-by-byte overlap semantics) -- from the chunk's token stream: packed literal
 // bytes + 4-byte {literal run, length, offset} records (format: ldb_common.cuh).
 //
-// B200 mapping -- ONE WARP per chunk, 32 single-warp CTAs per SM, no block barriers:
+// H100 mapping -- ONE WARP per chunk, 32 single-warp CTAs per SM, no block barriers:
 //   * LZ77 text has dependency chains hundreds of matches deep (every occurrence of a frequent
 //     word copies from the previous one), so the chunk is walked in order, 32 records (one per
 //     lane) at a time, and what counts is the latency of one dependent step and how many chunks
 //     an SM holds.  Shared memory per chunk: a 4 KiB staging ring in which the current group is
 //     assembled.  The 32 KiB window is the chunk's own committed output, read back through
-//     L1/L2 (148 x 32 windows of 32 KiB; the recently written part of each is what matches mostly
-//     reach for, and the 126 MB L2 holds it) (measured first with the
-//     window as a shared-memory ring: 36 KiB per chunk, 6 warps per SM, 0.14 IPC per warp --
-//     profiles/r02_inflate_b.md);
+//     L1/L2 (132 x 32 windows of 32 KiB; the recently written part of each is what matches mostly
+//     reach for, and the 50 MB L2 holds that part) (the window as a shared-memory ring would
+//     take 36 KiB per chunk and leave room for 6 warps per SM);
 //   * per group: two warp prefix sums ({literals}, {literals + length}) give every lane its
 //     literal source and its destination; all literal runs and all matches whose source lies in
 //     the window ("far": ~90 % of them) are copied by their own lanes at once, 16 bytes per step
@@ -24,8 +23,8 @@
 //     byte-by-byte overlap rule becomes index arithmetic: byte k comes from k mod offset);
 //   * finished 16-byte rows go staging -> global: coalesced 16-byte stores are the only global
 //     stores of the kernel.
-// (A block-parallel version with exact dependency tracking in rounds was measured first: 232 K
-// warp instructions per chunk, ~50 rounds per 256 records on Zipf text -- profiles/r02_inflate_a.md.)
+// (A block-parallel version with exact dependency tracking in rounds was the first design: it needs
+// ~50 rounds per 256 records on Zipf text.)
 //
 // Algorithmic HBM bytes per chunk: actual_out written once (+ the token stream read once, which
 // is the price of the two-kernel split; see inflate_kernel.cu).
@@ -50,7 +49,7 @@
 #define RES_LD_REC(p) __ldg(p)
 #endif
 #ifndef RES_PER_SM
-#define RES_PER_SM  32		// warps (= chunks) per SM; measured 8 / 16 / 24 / 32: 25.9 / 14.2 / 10.6 / 9.0 ms per 4 GiB
+#define RES_PER_SM  32		// warps (= chunks) per SM: as many as an SM holds CTAs, the walk is latency-bound
 #endif
 
 // the scratch slot of a chunk: what the decoder can emit is bounded both by the output room

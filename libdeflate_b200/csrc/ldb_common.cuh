@@ -1,6 +1,6 @@
 // ldb_common.cuh -- shared definitions for the libdeflate_b200 CUDA sources.
 //
-// Target: sm_100a only (B200).  No multi-backend dispatch, no CPU fallback.
+// Target: sm_90a only (H100).  No multi-backend dispatch, no CPU fallback.
 // When LDB_EMU is defined the same sources are compiled by g++ against
 // tests/emu/cuda_emu.h for CPU-side logic tests (test infrastructure only).
 #pragma once

@@ -1,6 +1,6 @@
 // shim.cu -- the C-ABI of libdeflate_b200: the 21 libdeflate.h symbols plus the
 // libdeflate_b200.h batch extension, implemented as thin host code around the
-// sm_100a kernels in this directory.  There is no CPU implementation of any
+// sm_90a kernels in this directory.  There is no CPU implementation of any
 // codec or checksum here: without a CUDA device every compute entry point fails
 // loudly (error text on stderr + abort for the classic API, error code for the
 // batch API).
@@ -36,7 +36,7 @@ extern "C" const char *libdeflate_b200_last_error(void) { return g_last_error; }
 [[noreturn]] static void ldb_die(const char *where)
 {
 	fprintf(stderr, "libdeflate_b200: FATAL in %s: %s\n"
-			"libdeflate_b200 has no CPU fallback; a CUDA device (B200, sm_100a) is required.\n",
+			"libdeflate_b200 has no CPU fallback; a CUDA device (H100, sm_90a) is required.\n",
 		where, g_last_error[0] ? g_last_error : "no CUDA device available");
 	abort();
 }
@@ -196,7 +196,7 @@ extern "C" struct libdeflate_b200_ctx *libdeflate_b200_ctx_create(int device)
 	ctx->stream = nullptr;
 	int v = 0;
 	cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device);
-	ctx->cfg.num_sms = v > 0 ? v : 148;
+	ctx->cfg.num_sms = v > 0 ? v : 132;
 	cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
 	ctx->cfg.max_smem_optin = v > 0 ? v : 232448;
 	if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||

@@ -1,4 +1,4 @@
-# End-of-round verification on one B200: smoke, GPU parity tests, DRAM traffic (ncu) for the roofline.traffic fields,
+# End-of-round verification on one GPU: smoke, GPU parity tests, DRAM traffic (ncu) for the roofline.traffic fields,
 # launch list of the default command, the default bench line (all legs) and the reference arm.
 mkdir -p gpurun_out
 timeout 600 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/f_smoke.log 2>&1; echo "smoke exit $?" >> gpurun_out/f_smoke.log

@@ -1,4 +1,4 @@
-# Last check of the round on one B200: smoke, the whole GPU suite, the default bench line (no profiler runs)
+# Last check of the round on one GPU: smoke, the whole GPU suite, the default bench line (no profiler runs)
 mkdir -p gpurun_out
 timeout 300 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/z_smoke.log 2>&1; echo "smoke exit $?" >> gpurun_out/z_smoke.log
 timeout 900 python -m pytest tests -m gpu -q > gpurun_out/z_pytest.log 2>&1; echo "pytest exit $?" >> gpurun_out/z_pytest.log

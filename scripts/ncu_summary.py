@@ -1,7 +1,7 @@
-"""Turns an .ncu-rep (brought back in gpurun_out/) into a small committed summary:
+"""Turns an .ncu-rep into a small text summary:
 key raw metrics + the top source lines by instructions and by stall samples.
 
-    python scripts/ncu_summary.py gpurun_out/prof_inflate3.ncu-rep profiles/r01_inflate
+    python scripts/ncu_summary.py prof_inflate.ncu-rep out/inflate
 """
 import csv
 import io

@@ -1,8 +1,7 @@
 """compute-sanitizer target: a handful of small chunks through every kernel (inflate decode + resolve,
 deflate at three levels, both checksums).  Run as
     compute-sanitizer --tool memcheck  python scripts/sanitize_small.py
-    compute-sanitizer --tool racecheck python scripts/sanitize_small.py
-and keep the log under profiles/."""
+    compute-sanitizer --tool racecheck python scripts/sanitize_small.py"""
 import os
 import sys
 import zlib

@@ -14,7 +14,8 @@ if len(sys.argv) > 4:
     bench.LEVEL = int(sys.argv[4])
 
 a = argparse.Namespace(gpus=1, steps=3, warmup=3, impl="b200", workload=sys.argv[2] if len(sys.argv) > 2 else "decompress",
-                       chunks=int(sys.argv[3]) if len(sys.argv) > 3 else 32768, chunk_size=int(sys.argv[5]) if len(sys.argv) > 5 else 65536, no_e2e=True, no_cpu=True, no_extra=True, no_l12=True, no_origin=True, data_class=0)
+                       chunks=int(sys.argv[3]) if len(sys.argv) > 3 else 32768, chunk_size=int(sys.argv[5]) if len(sys.argv) > 5 else 65536, no_e2e=True, no_cpu=True, no_extra=True, no_l12=True, no_origin=True, data_class=0,
+                       dump_outputs=None)
 bench.run_b200(a)
 try:
     ldb._lib.ldb_lz_timing_dump()

@@ -1,7 +1,7 @@
 """pytest plumbing.
 
-Markers:  gpu  -- needs a real B200 (run with `-m gpu` through gpurun).
-Everything else runs on CPU: the oracle against golden vectors / the real reference,
+Markers:  gpu  -- needs a CUDA device (an H100; `-m gpu` selects these tests).
+Everything else runs on CPU: the oracle against golden vectors / the reference's recorded answers,
 the host logic, symbol export checks, and the kernel LOGIC through the SIMT emulator
 (tests/emu, test infrastructure only -- never part of the product path).
 """
@@ -17,7 +17,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run via gpurun")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100)")
 
 
 def _have_gpu():
@@ -31,7 +31,7 @@ def _have_gpu():
 def pytest_collection_modifyitems(config, items):
     if _have_gpu():
         return
-    skip = pytest.mark.skip(reason="no CUDA device here (GPU tests run through gpurun)")
+    skip = pytest.mark.skip(reason="no CUDA device here")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)
@@ -91,18 +91,15 @@ def oracle():
     return Oracle()
 
 
-@pytest.fixture(scope="session")
-def reflib():
-    """The UNMODIFIED reference (oracle/_ref/libdeflate_ref.so) through the product's own
-    ctypes prototypes; skipped when it has not been built (it needs /root/reference)."""
-    import libdeflate_b200 as ldb
-    so = os.path.join(ROOT, "oracle", "_ref", "libdeflate_ref.so")
-    if not os.path.exists(so):
-        if os.path.isdir("/root/reference/lib"):
-            subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "ref"], stdout=subprocess.DEVNULL)
-        else:
-            pytest.skip("oracle/_ref not built and /root/reference absent")
-    return ldb.Api(_load_ref(so))
+@pytest.fixture
+def reflib(request):
+    """What the UNMODIFIED reference answered to this test's calls, replayed from
+    tests/golden/reference_calls.npz (recorded by tests/golden/make_fixtures.py)."""
+    import reference_calls
+    rp = reference_calls.replayer(request.node.name)
+    yield rp
+    if not request.session.testsfailed:
+        assert rp.i == len(rp.rows), "%s: %d of %d recorded reference calls made" % (rp.name, rp.i, len(rp.rows))
 
 
 def _load_ref(so):

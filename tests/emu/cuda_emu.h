@@ -6,8 +6,8 @@
 // sources* with g++ (-DLDB_EMU -include cuda_emu.h) and run every CUDA thread as
 // a cooperative fiber: one OS thread per resident block, one fiber per CUDA
 // thread, a context switch at every barrier / warp collective.  This checks the
-// kernel LOGIC (indexing, bit arithmetic, verdicts) on the CPU before a gpurun
-// call is spent.  It says nothing about performance and it is not a fallback:
+// kernel LOGIC (indexing, bit arithmetic, verdicts) on the CPU before GPU time
+// is spent.  It says nothing about performance and it is not a fallback:
 // the product library has no code path that reaches this header.
 //
 // Supported: threadIdx/blockIdx/blockDim/gridDim (x only... y/z = 0/1),

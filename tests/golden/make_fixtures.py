@@ -1,5 +1,6 @@
-"""Regenerates the committed golden fixtures.  Needs /root/reference (it runs the
-UNMODIFIED reference built into oracle/_ref/); the fixtures themselves travel with the repo.
+"""Regenerates the committed golden fixtures.  Needs the UNMODIFIED reference built into
+oracle/_ref/ (`make -C oracle ref REF=<reference source tree>`); the fixtures themselves travel
+with the repo.
 
     python tests/golden/make_fixtures.py
 
@@ -9,7 +10,14 @@ known_answer.json : hand-assembled raw-DEFLATE streams in the spirit of the refe
                     programs/test_incomplete_codes.c, test_invalid_streams.c, test_overread.c
                     and test_slow_decompression.c, with the verdict and output bytes the
                     reference returned for them here.
+reference_calls.npz: every answer the reference gave to the tests that compare against it
+                    (tests/reference_calls.py), recorded by running those tests here.
+ref_synth_streams.npz: the reference's level-6 gzip streams of the first SYNTH_CHUNKS chunks of
+                    bench/synth.c's robustness mix (all six classes T/P/S/R/Z/M), input of the
+                    full-size GPU test.
 """
+import ctypes
+import inspect
 import json
 import os
 import random
@@ -173,6 +181,53 @@ def known_answers():
         print("%-40s result=%d out=%d bytes" % (c["name"], c["result"], len(c["output"]) // 2))
 
 
+class _RefCtx:
+    """Batch calls answered chunk by chunk by the reference: runs a test body that needs a context without a device."""
+
+    def compress_batch_host(self, chunks, level=6, fmt=0, out_avail=None):
+        return [ref.compress(c, level, fmt, out_avail) for c in chunks]
+
+    def decompress_batch_host(self, streams, out_avail, fmt=0, exact=False):
+        avails = [out_avail] * len(streams) if isinstance(out_avail, int) else out_avail
+        return [ref.decompress(z, a, fmt, exact) for z, a in zip(streams, avails)]
+
+
+def reference_calls():
+    import reference_calls as rc
+    import test_emu_kernels
+    import test_gpu_parity
+    import test_oracle_pin
+    from conftest import Oracle
+    orc, ctx = Oracle(), _RefCtx()
+    tapes = {}
+    for mod in (test_oracle_pin, test_emu_kernels, test_gpu_parity):
+        for name, fn in sorted(vars(mod).items()):
+            if not name.startswith("test_") or "reflib" not in inspect.signature(fn).parameters:
+                continue
+            tapes[name] = rc.Recorder(ref)
+            have = {"oracle": orc, "reflib": tapes[name], "emu_ctx": ctx, "gpu_ctx": ctx}
+            fn(**{p: have[p] for p in inspect.signature(fn).parameters})
+            print("%-60s %d reference calls" % (name, len(tapes[name].rows)))
+    rc.save(tapes)
+
+
+SYNTH_CHUNKS = 31      # coprime to the 32 lanes of a warp; ~0.6 MB of streams, below the 1 MB file limit
+
+
+def synth_streams():
+    import bench
+    synth = bench.load_synth()
+    chunk, index = 65536, list(range(SYNTH_CHUNKS))   # class 6: chunk i is of class i % 6
+    arrs = {"index": np.array(index)}
+    for i in index:
+        buf = (ctypes.c_uint8 * chunk)()
+        synth.synth_fill(buf, chunk, i, 1, 6, 1)
+        arrs["z%d" % i] = np.frombuffer(ref.compress(bytes(buf), 6, 2), dtype=np.uint8)
+    np.savez_compressed(os.path.join(HERE, "ref_synth_streams.npz"), **arrs)
+
+
 if __name__ == "__main__":
     ref_streams()
     known_answers()
+    reference_calls()
+    synth_streams()

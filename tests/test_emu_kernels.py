@@ -15,8 +15,8 @@ def test_checksum_batch_emulated(emu_ctx, oracle):
     pc.check_checksum_batch(emu_ctx, oracle, n_chunks=40, max_len=20000)
 
 
-def test_inflate_valid_streams_emulated(emu_ctx, oracle, reflib):
-    streams = pc.make_valid_streams(sizes=(0, 1, 100, 5000, 40000), levels=(1, 6), ref=reflib)
+def test_inflate_valid_streams_emulated(emu_ctx, oracle):
+    streams = pc.make_valid_streams(sizes=(0, 1, 100, 5000, 40000), levels=(1, 6)) + pc.reference_fixture_streams(max_size=40000)
     pc.check_decompress_valid(emu_ctx, oracle, streams)
 
 
