@@ -175,7 +175,8 @@ libdeflate_b200_decompress_batch_host_packed(struct libdeflate_b200_ctx *ctx, in
 					     void *const *h_out, const size_t *h_out_avail,
 					     size_t *h_actual_in, size_t *h_actual_out, int32_t *h_results);
 /* Device-side packing (asynchronous): chunk i -> d_dense + d_offsets[i]; d_offsets has n + 1 entries,
- * the last one is the packed size; chunks that would not fit dense_avail are skipped. */
+ * the last one is the packed size (so n = 0 writes d_offsets[0] = 0); chunks that would not fit
+ * dense_avail are skipped, and chunks with a NULL pointer are not read. */
 LIBDEFLATEAPI int
 libdeflate_b200_pack_batch(struct libdeflate_b200_ctx *ctx, const void *const *d_ptrs, const size_t *d_sizes,
 			   size_t n_chunks, void *d_dense, size_t dense_avail, uint64_t *d_offsets);

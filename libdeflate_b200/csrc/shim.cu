@@ -863,8 +863,11 @@ extern "C" int libdeflate_b200_decompress_batch_host_packed(struct libdeflate_b2
 extern "C" int libdeflate_b200_pack_batch(struct libdeflate_b200_ctx *ctx, const void *const *d_ptrs, const size_t *d_sizes,
 					   size_t n, void *d_dense, size_t dense_avail, uint64_t *d_offsets)
 {
-	if (n == 0) return 0;
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	if (n == 0) {	// an empty batch packs to 0 bytes: d_offsets[0] says so, still without waiting
+		if (d_offsets) LDB_CUDA_CHECK_RET(cudaMemsetAsync(d_offsets, 0, sizeof(uint64_t), ctx->stream));
+		return 0;
+	}
 	ctx->launches++;	// offsets + copy
 	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_pack(d_ptrs, d_sizes, n, d_dense, dense_avail, (u64 *)d_offsets, ctx->cfg, ctx->stream); });
 }

@@ -87,6 +87,22 @@ def check_truncation_and_space_sweep(ctx, orc, n_text=6000):
     start, ref: lib/deflate_decompress.c:236-254) and the "no room" verdicts.  So: one text stream cut at every
     byte of its last 48 bytes (plus a spread of earlier cuts), zero-extended, and every output size from a few
     bytes short to a few bytes long -- verdict, byte counts and bytes against the oracle."""
+    streams, avails = truncation_sweep_cases(n_text)
+    for exact in (False, True):
+        got = ctx.decompress_batch_host(streams, avails, 0, exact)
+        seen = set()
+        for z, a, g in zip(streams, avails, got):
+            r = orc.decompress(z, a, 0, exact)
+            seen.add(r[0])
+            if r[0] == 0:
+                assert g == r, ("sweep mismatch", exact, len(z), a, g[0], g[2:], r[2:])
+            else:
+                assert g[0] == r[0], ("sweep verdict mismatch", exact, len(z), a, g[0], r[0])
+        assert seen >= {0, 1, 3}, seen
+
+
+def truncation_sweep_cases(n_text=6000):
+    """(raw streams, out_avail) of check_truncation_and_space_sweep."""
     plains = [corpus.text(n_text, 77), corpus.text(700, 78) + b"q" * 300 + corpus.text(500, 79), corpus.mixed(n_text, 80)]
     streams, avails = [], []
     for p in plains:
@@ -99,17 +115,7 @@ def check_truncation_and_space_sweep(ctx, orc, n_text=6000):
                 streams.append(z + bytes(extra)); avails.append(len(p))
             for d in (-9, -5, -4, -3, -2, -1, 1, 3):
                 streams.append(z); avails.append(max(0, len(p) + d))
-    for exact in (False, True):
-        got = ctx.decompress_batch_host(streams, avails, 0, exact)
-        seen = set()
-        for z, a, g in zip(streams, avails, got):
-            r = orc.decompress(z, a, 0, exact)
-            seen.add(r[0])
-            if r[0] == 0:
-                assert g == r, ("sweep mismatch", exact, len(z), a, g[0], g[2:], r[2:])
-            else:
-                assert g[0] == r[0], ("sweep verdict mismatch", exact, len(z), a, g[0], r[0])
-        assert seen >= {0, 1, 3}, seen
+    return streams, avails
 
 
 def check_decompress_large(ctx, sizes=(150000, 262144 + 123), levels=(0, 1, 6, 9)):
