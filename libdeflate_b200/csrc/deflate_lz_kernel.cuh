@@ -60,8 +60,22 @@
 #define LZ_MAX_DIST  (LZ_WIN - LZ_LOOKAHEAD)	// the oldest LOOKAHEAD bytes of the window are overwritten
 #define LZ_TOKCAP    (LZ_BLOCK_PASSES * LZ_PASS + 64)
 #define LZ_STAGE_WORDS 2048			// 8 KiB emission staging
-#define LZ_TPT         (LZ_THREADS > 512 ? 1 : 2)	// tokens per thread per emission round
-#define LZ_EMIT_ROUND  (LZ_THREADS * LZ_TPT)	// tokens per emission round (<= 48 bits each, <= 1536 words)
+// tokens per thread per emission round of a group of gt threads: <= 1024 tokens of <= 48 bits per
+// round (<= 1536 staging words)
+#define LZ_TPT(gt)     ((gt) > 512 ? 1u : 2u)
+// Levels 1-9 run two warp groups: warps [0, LZ_PWARPS) parse pass k and flush its block while the
+// others search pass k + 1, then join that search.  The block flush needs one thread per symbol of
+// the 320-symbol alphabets and of the <= 320 code lengths the precode run-length codes.  Deflate
+// kernel at L6, 65536 x 64 KiB on an H100 80GB HBM3 at a 400 W power limit: 10 / 12 / 14 / 16 warps
+// 293.0 / 288.6 / 287.8 / 294.8 ms (one-group order: 301.3 ms).
+#ifndef LZ_PWARPS
+#define LZ_PWARPS    14
+#endif
+#define LZ_BAR_P     1				// named barrier of the parse/flush group
+#ifndef LZ_PF
+#define LZ_PF        4				// parse: windows of per-position results in flight per warp
+#endif
+static_assert(LZ_PWARPS >= 10 && LZ_PWARPS < LZ_WARPS, "parse/flush group: 320..LZ_THREADS-32 threads");
 
 // shared memory layout
 #define LZ_SM_RING   0
@@ -111,7 +125,8 @@ struct lz_vars {
 	u32 obs_blk[8], obs_next[8];	// byte-class observations: current block / the pass after it
 	u32 end_early;		// the next pass looks different: end the block before it
 	u32 failed;
-	u32 obit_lo, obit_hi;	// output bit position (64-bit)
+	u32 obit_lo, obit_hi;	// output bit position (64-bit) } the parse/flush group's block state, published at
+	u32 blk_begin, blk_entry, blk_passes;	// block_begin, block_entry, pass_in_block  } every join
 	u32 pre_lens_packed[3];
 	u32 tma_phase;
 };
@@ -255,15 +270,15 @@ __device__ __forceinline__ void lz_stage_or(u32 *stage, u32 rel_bit, u64 bits, u
 	}
 }
 
-// Writes staging words [0, nwords) to the output at word index 'first_word'; all threads.
-__device__ __forceinline__ void lz_flush_words(const lz_out &o, const u32 *stage, u64 first_word, u32 nwords)
+// Writes staging words [0, nwords) to the output at word index 'first_word'; threads [0, nthreads).
+__device__ __forceinline__ void lz_flush_words(const lz_out &o, const u32 *stage, u64 first_word, u32 nwords, u32 nthreads)
 {
 	if ((((uintptr_t)o.out) & 3) == 0) {
 		u32 *dst = (u32 *)o.out + first_word;
-		for (u32 i = threadIdx.x; i < nwords; i += LZ_THREADS) dst[i] = stage[i];
+		for (u32 i = threadIdx.x; i < nwords; i += nthreads) dst[i] = stage[i];
 	} else {
 		u8 *dst = o.out + first_word * 4;
-		for (u32 i = threadIdx.x; i < nwords * 4; i += LZ_THREADS) dst[i] = (u8)(stage[i >> 2] >> (8 * (i & 3)));
+		for (u32 i = threadIdx.x; i < nwords * 4; i += nthreads) dst[i] = (u8)(stage[i >> 2] >> (8 * (i & 3)));
 	}
 }
 
@@ -318,11 +333,12 @@ __device__ __forceinline__ void lz_gen_codes_serial(const u8 *lens, u32 nsyms, u
 
 #ifdef LZ_TIMING
 #include <stdio.h>
-// tuning builds only: cycles per phase, summed over all CTAs (thread 0's clock between barriers;
-// the compiler may read the clock before the barrier wait, so a phase in which thread 0 finishes early
-// is under-counted and the wait shows up in the next one: read 'search phase' + 'parse e1' together)
-__device__ unsigned long long ldb_lz_timing[16];
-#define LZ_T(k) do { if (tid == 0) { long long t_ = clock64(); tacc[k] += t_ - tlast; tlast = t_; } } while (0)
+// tuning builds only: cycles per phase, summed over all CTAs, clocked separately by thread 0 (first
+// warp of the parse/flush group) and by the first thread of the search group; whole-CTA phases appear
+// in both.  (The compiler may read the clock before a barrier wait, so a phase in which the clocking
+// thread finishes early is under-counted and the wait shows up in the next one.)
+__device__ unsigned long long ldb_lz_timing[2][16];
+#define LZ_T(k) do { if (tid == 0 || tid == 32 * LZ_PWARPS) { long long t_ = clock64(); tacc[k] += t_ - tlast; tlast = t_; } } while (0)
 #else
 #define LZ_T(k) do { } while (0)
 #endif
@@ -683,10 +699,10 @@ __device__ void lz_dp_segment(const u8 *ring, const u32 *mlist, u32 *costg, u32 
 // Here blocks end on pass boundaries, so the test runs once per pass, on the bytes of the pass that
 // would join the block: lz_observe() counts their classes (all threads), lz_should_end_block()
 // applies the reference's integer arithmetic to the two histograms.
-__device__ __forceinline__ void lz_observe(const u8 *ring, u32 from, u32 to, u32 *obs, u32 tid, u32 lane)
+__device__ __forceinline__ void lz_observe(const u8 *ring, u32 from, u32 to, u32 *obs, u32 tid, u32 lane, u32 nthreads)
 {
 	// 16 bytes per thread and round; class counts in 8 packed byte fields, reduced per warp
-	for (u32 wbase = from + 512 * (tid >> 5); wbase < to; wbase += 16 * LZ_THREADS) {	// warp-uniform trip count
+	for (u32 wbase = from + 512 * (tid >> 5); wbase < to; wbase += 16 * nthreads) {	// warp-uniform trip count
 		const u32 base = wbase + 16 * lane;
 		const uint4 q = *(const uint4 *)(ring + (base & (LZ_RING - 1)));	// from is 16 KiB aligned
 		const u32 w[4] = {q.x, q.y, q.z, q.w};
@@ -761,6 +777,17 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 	long long tlast = clock64();
 #endif
 	const lz_params P = lz_level_params(a.level);
+	// Levels 1-9 (pipe): warps [0, LZ_PWARPS) parse pass k and flush its block while the other warps
+	// search pass k + 1 (nothing the parse and the flush read is written by that search); the last
+	// pass of a chunk, with nothing left to search, is parsed and flushed by the whole CTA.  Levels
+	// 10-12 need the whole block for the min-cost path and run in order on the whole CTA.  GW / GT:
+	// warps / threads of the group that parses and flushes (warp 0 up), gsync() its barrier.
+	const bool pipe = !P.opt_iters;
+	u32 GW = LZ_WARPS, GT = LZ_THREADS;
+	auto gsync = [&]() {
+		if (GT < LZ_THREADS) LDB_BAR_SYNC(LZ_BAR_P, GT);
+		else __syncthreads();
+	};
 
 	if (tid == 0) {
 		v->tma_phase = 0;
@@ -841,33 +868,35 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 
 		// ---- exact parallel parse of one pass (positions [pb0, ppend), results at res[aoff + i]).
 		// forced: the DP already decided (flag set on matches); otherwise the lazy rule decides.
-		// exitt: 16 Ki u16 of scratch in shared memory -- the link slots of the first pass that is not
-		// inserted yet (dead, see lz_insert_pass_par)
+		// exitt: 16 Ki u16 of scratch in shared memory -- dead link slots (see lz_insert_pass_par and the
+		// pass loop below)
 		auto parse_pass = [&](const u32 pb0, const u32 ppend, const u32 aoff, const bool forced, u16 *exitt) {
 			// (e1) per-window decisions + "exit position for every entry lane" by pointer jumping
 			const u32 nwin = (ppend - pb0 + 31) >> 5;
-			// (the per-position results live in L2: the loads run two windows ahead of their use)
+			// (the per-position results live in L2: every warp walks its contiguous group of windows
+			// [wbeg, wend) -- the groups of e2 -- with the loads of LZ_PF windows in flight, and the last
+			// lane takes the next window's first two results from those loads by shuffle)
 			const u32 min_len = v->min_len, far4 = v->far4_dist;
-			auto e1_load = [&](u32 w, u32 &x0, u32 &x1, u32 &x2) {
-				x0 = 0; x1 = 0; x2 = 0;
-				if (w < nwin) {
-					const u32 i = w * 32 + lane;
-					if (pb0 + i < ppend) x0 = res[aoff + i];
-					if (lane == 31 && pb0 + i + 1 < ppend) x1 = res[aoff + i + 1];	// (the others get it by shuffle)
-					if (lane == 31 && P.lazy == 2 && pb0 + i + 2 < ppend) x2 = res[aoff + i + 2];
-				}
+			const u32 G = (nwin + GW - 1) / GW;			// windows per group
+			const u32 wbeg = warp * G, wend = wbeg + G < nwin ? wbeg + G : nwin;
+			auto res_load = [&](u32 w) -> u32 {
+				const u32 i = w * 32 + lane;
+				return w < nwin && pb0 + i < ppend ? res[aoff + i] : 0;
 			};
-			u32 cW0, cW1, cW2, nW0, nW1, nW2;
-			e1_load(warp, cW0, cW1, cW2);
-			e1_load(warp + LZ_WARPS, nW0, nW1, nW2);
-			for (u32 w = warp; w < nwin; w += LZ_WARPS) {
+			u32 q[LZ_PF];
+#pragma unroll
+			for (int k = 0; k < LZ_PF; k++) q[k] = res_load(wbeg + k);
+			for (u32 w = wbeg; w < wend; w++) {
 				u32 i = w * 32 + lane;
 				u32 p = pb0 + i;
-				const u32 W0 = cW0, nb = __shfl_down_sync(LDB_FULL_MASK, W0, 1), W1 = lane == 31 ? cW1 : nb;
-				const u32 nb2 = __shfl_down_sync(LDB_FULL_MASK, W1, 1), W2 = lane == 31 ? cW2 : nb2;	// two ahead (lazy2)
+				const u32 W0 = q[0], nx = q[1];
+#pragma unroll
+				for (int k = 0; k + 1 < LZ_PF; k++) q[k] = q[k + 1];
+				q[LZ_PF - 1] = res_load(w + LZ_PF);
+				const u32 nx0 = __shfl_sync(LDB_FULL_MASK, nx, 0), nx1 = __shfl_sync(LDB_FULL_MASK, nx, 1);
+				const u32 nb = __shfl_down_sync(LDB_FULL_MASK, W0, 1), W1 = lane == 31 ? nx0 : nb;
+				const u32 nb2 = __shfl_down_sync(LDB_FULL_MASK, W1, 1), W2 = lane == 31 ? nx1 : nb2;	// two ahead (lazy2)
 				const u32 L0 = W0 & 0xffff, O0 = ((W0 >> 16) & 0x7fff) + 1, L1 = W1 & 0xffff, O1 = ((W1 >> 16) & 0x7fff) + 1;
-				cW0 = nW0; cW1 = nW1; cW2 = nW2;
-				e1_load(w + 2 * LZ_WARPS, nW0, nW1, nW2);
 				// (a shortest-possible match at a long distance costs more bits than its literals: the
 				// reference's rule for length 3 beyond 8 KiB, deflate_compress.c:2666-2668, restated for our
 				// minimum length 4)
@@ -898,16 +927,15 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				}
 				if (p < ppend) exitt[i] = (u16)j;
 			}
-			__syncthreads();
+			gsync();
 			LZ_T(8);
 			// (e2) chain the windows.  A serial walk over all windows costs ~300 cycles per window on
 			// one warp, so it is split: (a) every warp composes the exits of ITS group of windows for
 			// all 32 possible entry lanes of the group's first window (per-lane shuffles), (b) warp 0
-			// chains the 16 groups, (c) every warp re-walks its group along the one real trajectory and
+			// chains the groups, (c) every warp re-walks its group along the one real trajectory and
 			// records the entry lane of each window.
 			{
-				const u32 G = (nwin + LZ_WARPS - 1) / LZ_WARPS;		// windows per group
-				const u32 wg0 = warp * G;				// first window of my group
+				const u32 wg0 = wbeg;				// first window of my group
 				const u32 gstart = wg0 * 32;				// pass-relative position
 				// (a) exits of the group for entries gstart + lane
 				{
@@ -929,11 +957,11 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					}
 					gexit[warp * 32 + lane] = (u16)(pos > 0xffff ? 0xffff : pos);
 				}
-				__syncthreads();
+				gsync();
 				// (b) chain the groups (warp 0, all lanes redundantly; lane 0 publishes)
 				if (warp == 0) {
 					u32 e = v->parse_entry - pb0;	// pass-relative
-					for (u32 g = 0; g < LZ_WARPS; g++) {
+					for (u32 g = 0; g < GW; g++) {
 						const u32 gs = g * G * 32, ge = (g + 1) * G * 32;
 						u32 ent = 0xffffffffu;
 						if (e < ge && gs < (nwin << 5) && pb0 + e < ppend) {
@@ -958,7 +986,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					__syncwarp();	// every lane has read parse_entry (racecheck: read/write by different lanes)
 					if (lane == 0) v->parse_entry = fin;
 				}
-				__syncthreads();
+				gsync();
 				// (c) entry lane of every window of my group along the real trajectory
 				{
 					u32 pos = gentry[warp];
@@ -983,24 +1011,20 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					}
 				}
 			}
-			__syncthreads();
+			gsync();
 			LZ_T(9);
-			// (e3) visited sets per window (the loads of the next window are issued first)
-			auto e3_load = [&](u32 w, u32 &e, u32 &x) {
-				e = 0xff; x = 0;
-				if (w < nwin) {
-					const u32 i = w * 32 + lane;
-					e = entryt[w];
-					if (e != 0xff && pb0 + i < ppend) x = res[aoff + i];
-				}
+			// (e3) visited sets per window (loads in flight as in e1)
+			auto e3_load = [&](u32 w) -> u32 {
+				const u32 i = w * 32 + lane;
+				return w < nwin && entryt[w] != 0xff && pb0 + i < ppend ? res[aoff + i] : 0;
 			};
-			u32 e3_e, e3_w, e3_ne, e3_nw;
-			e3_load(warp, e3_e, e3_w);
-			e3_load(warp + LZ_WARPS, e3_ne, e3_nw);
-			for (u32 w = warp; w < nwin; w += LZ_WARPS) {
-				const u32 e = e3_e, rw = e3_w;
-				e3_e = e3_ne; e3_w = e3_nw;
-				e3_load(w + 2 * LZ_WARPS, e3_ne, e3_nw);
+#pragma unroll
+			for (int k = 0; k < LZ_PF; k++) q[k] = e3_load(wbeg + k);
+			for (u32 w = wbeg; w < wend; w++) {
+				const u32 e = entryt[w], rw = q[0];
+#pragma unroll
+				for (int k = 0; k + 1 < LZ_PF; k++) q[k] = q[k + 1];
+				q[LZ_PF - 1] = e3_load(w + LZ_PF);
 				u32 V = 0;
 				if (e != 0xff) {
 					u32 step = (rw & 0x80000000u) ? (rw & 0xffff) : 1;
@@ -1024,7 +1048,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				}
 				if (lane == 0) vis[w] = V;
 			}
-			__syncthreads();
+			gsync();
 			LZ_T(10);
 			// (e4) token offsets (exclusive scan over windows) by warp 0
 			if (warp == 0) {
@@ -1042,25 +1066,21 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				}
 				if (lane == 0) tokoff[LZ_NWIN] = run;
 			}
-			__syncthreads();
+			gsync();
 			LZ_T(11);
 			// (e5) emit tokens + histograms
 			const u32 tbase = v->tok_count;
-			auto e5_load = [&](u32 w, u32 &V, u32 &x) {
-				V = 0; x = 0;
-				if (w < nwin) {
-					V = vis[w];
-					if ((V >> lane) & 1) x = res[aoff + w * 32 + lane];
-				}
+			auto e5_load = [&](u32 w) -> u32 {
+				return w < nwin && ((vis[w] >> lane) & 1) ? res[aoff + w * 32 + lane] : 0;
 			};
-			u32 e5_V, e5_w, e5_nV, e5_nw;
-			e5_load(warp, e5_V, e5_w);
-			e5_load(warp + LZ_WARPS, e5_nV, e5_nw);
-			for (u32 w = warp; w < nwin; w += LZ_WARPS) {
-				const u32 V = e5_V, ro = e5_w >> 16;
-				const u32 len = e5_w & 0xffff;
-				e5_V = e5_nV; e5_w = e5_nw;
-				e5_load(w + 2 * LZ_WARPS, e5_nV, e5_nw);
+#pragma unroll
+			for (int k = 0; k < LZ_PF; k++) q[k] = e5_load(wbeg + k);
+			for (u32 w = wbeg; w < wend; w++) {
+				const u32 V = vis[w], ro = q[0] >> 16;
+				const u32 len = q[0] & 0xffff;
+#pragma unroll
+				for (int k = 0; k + 1 < LZ_PF; k++) q[k] = q[k + 1];
+				q[LZ_PF - 1] = e5_load(w + LZ_PF);
 				if (!V) continue;
 				u32 i = w * 32 + lane;
 				if ((V >> lane) & 1) {
@@ -1078,9 +1098,9 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					}
 				}
 			}
-			__syncthreads();
+			gsync();
 			if (tid == 0) v->tok_count = tbase + tokoff[LZ_NWIN];
-			__syncthreads();
+			gsync();
 		};
 
 		// ---- Huffman codes from freq[] -> lens[], codes[] (all threads)
@@ -1091,20 +1111,20 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				u32 t = __shfl_up_sync(LDB_FULL_MASK, incl, o2);
 				if (lane >= (u32)o2) incl += t;
 			}
-			__syncthreads();		// earlier readers of escan are done
+			gsync();		// earlier readers of escan are done
 			if (lane == 31) escan[warp] = incl;
-			__syncthreads();
+			gsync();
 			if (warp == 0) {
-				u32 y = lane < LZ_WARPS ? escan[lane] : 0;
+				u32 y = lane < GW ? escan[lane] : 0;
 				u32 yi = y;
 				for (int o2 = 1; o2 < 32; o2 <<= 1) {
 					u32 t = __shfl_up_sync(LDB_FULL_MASK, yi, o2);
 					if (lane >= (u32)o2) yi += t;
 				}
-				if (lane < LZ_WARPS) escan[32 + lane] = yi - y;
-				if (lane == LZ_WARPS - 1) escan[64] = yi;
+				if (lane < GW) escan[32 + lane] = yi - y;
+				if (lane == GW - 1) escan[64] = yi;
 			}
-			__syncthreads();
+			gsync();
 			total = escan[64];
 			return escan[32 + warp] + (incl - x);
 		};
@@ -1118,7 +1138,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			const u32 lo = is_lit ? 0 : 288, hi = is_lit ? 288 : 320;
 			if (tid == 0) { v->nused_lit = 0; v->nused_off = 0; v->huff_over = 0; }
 			if (tid < 34) hcount[tid] = 0;
-			__syncthreads();
+			gsync();
 			u32 myrank = 0xffffffffu;
 			if (tid < 320) {
 				const u32 f = freq[tid];
@@ -1135,11 +1155,11 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					atomicAdd(is_lit ? &v->nused_lit : &v->nused_off, 1u);
 				}
 			}
-			__syncthreads();
+			gsync();
 			const u32 nused = is_lit ? v->nused_lit : v->nused_off;
 			if (tid == 0 && nused >= 2) lz_huffman_merge(hnodefreq, hparent, nused);
 			if (tid == 32) { const u32 nu = v->nused_off; if (nu >= 2) lz_huffman_merge(onodefreq, oparent, nu); }
-			__syncthreads();
+			gsync();
 			if (tid < 320 && myrank != 0xffffffffu && nused >= 2) {
 				const u16 *par = is_lit ? hparent : oparent;
 				const u32 root = 2 * nused - 2;
@@ -1148,7 +1168,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				if (d > 15) { d = 15; v->huff_over = 1; }
 				atomicAdd(&(is_lit ? hcount : ocount)[d], 1u);
 			}
-			__syncthreads();
+			gsync();
 			if ((tid == 0 || tid == 288) && nused < 2) {
 				// at least two codewords (ref: deflate_compress.c:1369-1378)
 				u8 *ln = lens + lo;
@@ -1171,7 +1191,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					kraft -= 1;
 				}
 			}
-			__syncthreads();
+			gsync();
 			if (tid < 320 && myrank != 0xffffffffu && nused >= 2) {
 				// rarest symbols get the longest codes
 				const u32 *cn = is_lit ? hcount : ocount;
@@ -1182,7 +1202,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				}
 				lens[tid] = (u8)len;
 			}
-			__syncthreads();
+			gsync();
 			if (tid < 320) {
 				const u32 l = lens[tid];
 				u32 code = 0;
@@ -1196,7 +1216,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				}
 				codes[tid] = (u16)code;
 			}
-			__syncthreads();
+			gsync();
 		};
 
 		u32 loaded_end = 0;
@@ -1204,182 +1224,122 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		u32 block_entry = 0;	// position of the first token of the current block
 		u32 pass_in_block = 0;
 
-		for (u32 b0 = 0; b0 < n; b0 += LZ_PASS) {
-			const u32 pend = b0 + LZ_PASS < n ? b0 + LZ_PASS : n;
-			const bool last = pend >= n;
-			if (tid == 0) v->run_counter = 0;
-			__syncthreads();
-			// (a) window staging by the TMA engine, one pass ahead: searching this pass needs
-			// [b0 - MAX_DIST, pend + LOOKAHEAD), inserting the next one (concurrently) needs the
-			// bytes up to pend + PASS + 3.  The ring then still holds everything back to
-			// b0 - 32768 + 16, i.e. the whole MAX_DIST window.
-			{
-				const u32 want = pend + LZ_PASS + 16 < n ? pend + LZ_PASS + 16 : n;
-				while (loaded_end < want) {
-					u32 room = LZ_RING - (loaded_end & (LZ_RING - 1));	// a segment must not wrap
-					u32 to = loaded_end + (room < LZ_SEG ? room : LZ_SEG);
-					if (to > want) to = want;
-					lz_load_segment(sm, v, in, loaded_end, to);
-					loaded_end = to;
-				}
-			}
-			if (b0 == 0) {
-				// alphabet size of the first 4 KiB -> minimum match length (ref:
-				// calculate_min_match_len, lib/deflate_compress.c:2329-2346)
-				if (tid < 8) { v->used_lits[tid] = 0; v->obs_blk[tid] = 0; }
-				__syncthreads();
-				lz_observe(ring, 0, pend, v->obs_blk, tid, lane);
-				const u32 scan = n < 4096 ? n : 4096;
-				for (u32 i = tid; i < scan; i += LZ_THREADS) {
-					u32 bv = ring[i];
-					atomicOr(&v->used_lits[bv >> 5], 1u << (bv & 31));
-				}
-				__syncthreads();
-				if (tid == 0) {
-					u32 cnt = 0;
-					for (int k = 0; k < 8; k++) cnt += __popc(v->used_lits[k]);
-					v->min_len = n < 512 ? 4 : lz_choose_min_len(cnt, (u32)P.depth);
-					// few distinct byte values = cheap literals (text): a far 4-byte match loses against them
-					v->far4_dist = cnt < 80 ? LZ_FAR4_DIST : LZ_WIN;
-				}
-				__syncthreads();
-			}
-			// (b) the whole CTA links this pass into the hash chains (ordered within a hash)
-			LZ_T(0);	// loads + first-pass extras
-#ifdef LZ_TIMING
-			lz_insert_pass_par(ring, head, nextt, (u32 *)(sm + LZ_SM_R), b0, pend, n, tid, lane, warp, tacc, tlast);
-#else
-			lz_insert_pass_par(ring, head, nextt, (u32 *)(sm + LZ_SM_R), b0, pend, n, tid, lane, warp);
-#endif
-			LZ_T(3);	// insertion: linking
-			{
-				// (c) guided search.  Every searcher owns a run of consecutive positions and walks
-				// it like the reference's lazy parser (deflate_compress.c:2605-2808): search where
-				// a token could start, look one position ahead, then skip the positions the
-				// chosen match covers (they inherit it at the same distance).  Every position
-				// still gets a (length, distance), so the exact parallel parse below can start a
-				// token anywhere.  One search call site per loop trip keeps the warp converged.
-				u32 *rs = res + pass_in_block * LZ_PASS;
-				if (P.opt_iters) {
-					// levels 10-12: every position is searched and keeps its list of matches
-					for (u32 i = tid; b0 + i < pend; i += LZ_THREADS) {
-						const u32 p = b0 + i;
-						u32 L = 0, D = 0;
-						u32 *ml = mlist + (size_t)(pass_in_block * LZ_PASS + i) * LZ_OPT_K;
-						if (p + 4 <= n) {
-							lz_search_all(ring, nextt, p, n, P.depth, (u32)P.nice, ml, L, D);
-						} else {
-							for (u32 k = 0; k < LZ_OPT_K; k++) ml[k] = 0;
-						}
-						rs[i] = L ? L | ((D - 1) << 16) : 0;
-					}
-				} else {
-				const u32 min_len = v->min_len, far4 = v->far4_dist;
-				// A run starts its walk without knowing where the parse really enters it, so short
-				// runs cost a little ratio (L6: +0.9 % at 16 vs 32) and buy parallelism; the deep
-				// levels, which are chosen for ratio, keep 32.
+		// ---- guided search of pass [b0, pend) -> rs[] (levels 1-9; any set of threads, any number of
+		// times: runs are handed out by v->run_counter and each run's results depend on the run alone)
+		auto search_pass = [&](const u32 b0, const u32 pend, u32 *rs) {
+			// (c) guided search.  Every searcher owns a run of consecutive positions and walks
+			// it like the reference's lazy parser (deflate_compress.c:2605-2808): search where
+			// a token could start, look one position ahead, then skip the positions the
+			// chosen match covers (they inherit it at the same distance).  Every position
+			// still gets a (length, distance), so the exact parallel parse below can start a
+			// token anywhere.  One search call site per loop trip keeps the warp converged.
+			const u32 min_len = v->min_len, far4 = v->far4_dist;
+			// A run starts its walk without knowing where the parse really enters it, so short
+			// runs cost a little ratio (L6: +0.9 % at 16 vs 32) and buy parallelism; the deep
+			// levels, which are chosen for ratio, keep 32.
 #ifndef LZ_RUN_SHORT
 #define LZ_RUN_SHORT 16
 #endif
-				const u32 run_len = a.level >= 7 ? 32 : LZ_RUN_SHORT;
-				// runs are handed out dynamically (shared counter): lanes whose runs are cheap
-				// (long matches, few searches) take more of them, which keeps the warp busy
-				u32 i = 0, i_end = 0;
-				u32 pL = 0, pD = 0;		// pending match at position i-pending (lazy evaluation in progress)
-				u32 pending = 0;		// 0: none, 1: looking one position ahead, 2: two positions (lazy2)
+			const u32 run_len = a.level >= 7 ? 32 : LZ_RUN_SHORT;
+			// runs are handed out dynamically (shared counter): lanes whose runs are cheap
+			// (long matches, few searches) take more of them, which keeps the warp busy
+			u32 i = 0, i_end = 0;
+			u32 pL = 0, pD = 0;		// pending match at position i-pending (lazy evaluation in progress)
+			u32 pending = 0;		// 0: none, 1: looking one position ahead, 2: two positions (lazy2)
 #if LZ_QUANTUM
-				lz_walk wk;
-				wk.left = 0; wk.best_len = 0; wk.best_dist = 0; wk.cand = 0; wk.prev_dist = 0; wk.tailo = 0; wk.tailv = 0; wk.cur = 0;
-				bool in_search = false;
+			lz_walk wk;
+			wk.left = 0; wk.best_len = 0; wk.best_dist = 0; wk.cand = 0; wk.prev_dist = 0; wk.tailo = 0; wk.tailv = 0; wk.cur = 0;
+			bool in_search = false;
 #endif
-				for (;;) {
+			for (;;) {
 #if LZ_QUANTUM
-					if (!in_search) {
+				if (!in_search) {
 #endif
-					if (i >= i_end || b0 + i >= pend) {
-						const u32 r = atomicAdd(&v->run_counter, 1u);
-						i = r * run_len;
-						if (b0 + i >= pend || i >= LZ_PASS) break;
-						i_end = i + run_len;
+				if (i >= i_end || b0 + i >= pend) {
+					const u32 r = atomicAdd(&v->run_counter, 1u);
+					i = r * run_len;
+					if (b0 + i >= pend || i >= LZ_PASS) break;
+					i_end = i + run_len;
+					pending = 0;
+				}
+#if LZ_QUANTUM
+					const u32 p0 = b0 + i;
+					wk.best_len = 0; wk.best_dist = 0; wk.left = 0;
+					if (p0 + 4 <= n) {
+						u32 sL = 0, sD = 0;
+						if (pending) { sL = pL - pending >= 4 ? pL - pending : 0; sD = pD; }
+						lz_walk_setup(ring, nextt, p0, n, P.depth >> pending, (u32)P.nice, sL, sD, wk);
+					}
+					in_search = true;
+				}
+				lz_walk_steps(ring, nextt, b0 + i, n, (u32)P.nice, wk, LZ_QUANTUM);
+				if (wk.left > 0) continue;		// the others move on; this search resumes next trip
+				in_search = false;
+				const u32 p = b0 + i;
+				u32 L = wk.best_len, D = wk.best_dist;
+#else
+				const u32 p = b0 + i;
+				u32 L = 0, D = 0;
+				if (p + 4 <= n) {
+					if (pending) { L = pL - pending >= 4 ? pL - pending : 0; D = pD; }	// the pending match continues here
+					lz_search(ring, nextt, p, n, P.depth >> pending, (u32)P.nice, L, D);
+				}
+#endif
+				rs[i] = L ? L | ((D - 1) << 16) : 0;
+				u32 mpos, mL, mD;	// match to accept this trip (mL == 0: none)
+				if (pending) {
+					// ref: deflate_compress.c:2722-2725 (margin 2, one ahead), :2757-2760 (margin 6, two ahead)
+					const int margin = pending == 1 ? 2 : 6;
+					if (L >= pL && 4 * ((int)L - (int)pL) + ((int)(31 - __clz((int)pD)) - (int)(31 - __clz((int)D))) > margin) {
+						// the lookahead match is clearly better: literal(s) before i, keep looking
+						// ahead from i unless it is long enough to take at once
+						mpos = i; mL = L >= (u32)P.nice ? L : 0; mD = D;
+						if (!mL) { pL = L; pD = D; }
+						pending = mL == 0 ? 1 : 0;
+					} else if (pending == 1 && P.lazy == 2 && i + 1 < i_end && b0 + i + 1 < pend) {
+						pending = 2;
+						mpos = i; mL = 0; mD = 0;
+					} else {
+						mpos = i - pending; mL = pL; mD = pD;
 						pending = 0;
 					}
-#if LZ_QUANTUM
-						const u32 p0 = b0 + i;
-						wk.best_len = 0; wk.best_dist = 0; wk.left = 0;
-						if (p0 + 4 <= n) {
-							u32 sL = 0, sD = 0;
-							if (pending) { sL = pL - pending >= 4 ? pL - pending : 0; sD = pD; }
-							lz_walk_setup(ring, nextt, p0, n, P.depth >> pending, (u32)P.nice, sL, sD, wk);
-						}
-						in_search = true;
-					}
-					lz_walk_steps(ring, nextt, b0 + i, n, (u32)P.nice, wk, LZ_QUANTUM);
-					if (wk.left > 0) continue;		// the others move on; this search resumes next trip
-					in_search = false;
-					const u32 p = b0 + i;
-					u32 L = wk.best_len, D = wk.best_dist;
-#else
-					const u32 p = b0 + i;
-					u32 L = 0, D = 0;
-					if (p + 4 <= n) {
-						if (pending) { L = pL - pending >= 4 ? pL - pending : 0; D = pD; }	// the pending match continues here
-						lz_search(ring, nextt, p, n, P.depth >> pending, (u32)P.nice, L, D);
-					}
-#endif
-					rs[i] = L ? L | ((D - 1) << 16) : 0;
-					u32 mpos, mL, mD;	// match to accept this trip (mL == 0: none)
-					if (pending) {
-						// ref: deflate_compress.c:2722-2725 (margin 2, one ahead), :2757-2760 (margin 6, two ahead)
-						const int margin = pending == 1 ? 2 : 6;
-						if (L >= pL && 4 * ((int)L - (int)pL) + ((int)(31 - __clz((int)pD)) - (int)(31 - __clz((int)D))) > margin) {
-							// the lookahead match is clearly better: literal(s) before i, keep looking
-							// ahead from i unless it is long enough to take at once
-							mpos = i; mL = L >= (u32)P.nice ? L : 0; mD = D;
-							if (!mL) { pL = L; pD = D; }
-							pending = mL == 0 ? 1 : 0;
-						} else if (pending == 1 && P.lazy == 2 && i + 1 < i_end && b0 + i + 1 < pend) {
-							pending = 2;
-							mpos = i; mL = 0; mD = 0;
-						} else {
-							mpos = i - pending; mL = pL; mD = pD;
-							pending = 0;
-						}
-					} else if (L >= min_len && !(L == 4 && D > far4)) {
-						if (P.lazy && L < (u32)P.nice && i + 1 < i_end && b0 + i + 1 < pend) {
-							pending = 1; pL = L; pD = D;
-							mpos = i; mL = 0; mD = 0;
-						} else {
-							mpos = i; mL = L; mD = D;
-						}
-					} else {
+				} else if (L >= min_len && !(L == 4 && D > far4)) {
+					if (P.lazy && L < (u32)P.nice && i + 1 < i_end && b0 + i + 1 < pend) {
+						pending = 1; pL = L; pD = D;
 						mpos = i; mL = 0; mD = 0;
-					}
-					if (mL) {
-						// positions covered by the accepted match inherit it at the same distance;
-						// 'mend' (end of the match at that distance) only moves forward, so extending
-						// the inherited matches (needed when the match was capped at 258) is O(1) amortised
-						u32 stop = mpos + mL < i_end ? mpos + mL : i_end;
-						if (b0 + stop > pend) stop = pend - b0;
-						u32 mend = b0 + mpos + mL;
-						for (u32 k = i + 1; k < stop; k++) {
-							const u32 pk = b0 + k;
-							// (the match ended on a mismatch unless it was capped at 258 bytes)
-							if (mL == 258)
-								while (mend < n && mend - pk < 258 && lz_ld8(ring, mend) == lz_ld8(ring, mend - mD)) mend++;
-							u32 lk = mend - pk;
-							rs[k] = lk >= 4 ? lk | ((mD - 1) << 16) : 0;
-						}
-						i = mpos + mL;
 					} else {
-						i++;
+						mpos = i; mL = L; mD = D;
 					}
+				} else {
+					mpos = i; mL = 0; mD = 0;
 				}
-				}	// guided search (levels 1-9)
+				if (mL) {
+					// positions covered by the accepted match inherit it at the same distance;
+					// 'mend' (end of the match at that distance) only moves forward, so extending
+					// the inherited matches (needed when the match was capped at 258) is O(1) amortised
+					u32 stop = mpos + mL < i_end ? mpos + mL : i_end;
+					if (b0 + stop > pend) stop = pend - b0;
+					u32 mend = b0 + mpos + mL;
+					for (u32 k = i + 1; k < stop; k++) {
+						const u32 pk = b0 + k;
+						// (the match ended on a mismatch unless it was capped at 258 bytes)
+						if (mL == 258)
+							while (mend < n && mend - pk < 258 && lz_ld8(ring, mend) == lz_ld8(ring, mend - mD)) mend++;
+						u32 lk = mend - pk;
+						rs[k] = lk >= 4 ? lk | ((mD - 1) << 16) : 0;
+					}
+					i = mpos + mL;
+				} else {
+					i++;
+				}
 			}
-			__syncthreads();
-			LZ_T(1);	// search phase (barrier to barrier)
-			// (e) exact parallel parse of this pass -> tokens + histograms
-			parse_pass(b0, pend, pass_in_block * LZ_PASS, false, nextt + ((b0 + LZ_PASS) & 0xffff));
+		};
+
+		// ---- parse pass [b0, pend) (search results at res[aoff..]), end the block there or not, and flush
+		// it if it ends (group [0, GT)).  A block that does not fit the output sets v->failed.
+		auto parse_and_flush = [&](const u32 b0, const u32 pend, const u32 aoff, u16 *exitt) {
+			const bool last = pend >= n;
+			parse_pass(b0, pend, aoff, false, exitt);
 			LZ_T(2);	// parse
 			// ---- block boundary: every LZ_BLOCK_PASSES passes, or at the end of the input --------
 			// A block also ends early when the bytes of the next pass look different from the block
@@ -1387,15 +1347,15 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			pass_in_block++;
 			if (!last) {
 				if (tid < 8) v->obs_next[tid] = 0;
-				__syncthreads();
-				lz_observe(ring, pend, pend + LZ_PASS < n ? pend + LZ_PASS : n, v->obs_next, tid, lane);
-				__syncthreads();
+				gsync();
+				lz_observe(ring, pend, pend + LZ_PASS < n ? pend + LZ_PASS : n, v->obs_next, tid, lane, GT);
+				gsync();
 				if (tid == 0) v->end_early = lz_should_end_block(v->obs_blk, v->obs_next, pend - block_begin) ? 1 : 0;
-				__syncthreads();
+				gsync();
 				const bool end_now = pass_in_block == LZ_BLOCK_PASSES || v->end_early;
-				__syncthreads();
+				gsync();
 				if (tid < 8) v->obs_blk[tid] = end_now ? v->obs_next[tid] : v->obs_blk[tid] + v->obs_next[tid];
-				if (!end_now) continue;
+				if (!end_now) return;
 			}
 			const u32 npass_block = pass_in_block;
 			pass_in_block = 0;
@@ -1407,10 +1367,10 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			// (one warp each); the resulting choices are re-parsed by the same parallel parser.
 			for (int it = 0; it < P.opt_iters; it++) {
 				if (tid == 0) freq[256] = 1;
-				__syncthreads();
+				gsync();
 				build_codes();
 				// bit costs: unused symbols get a pessimistic default (cf. deflate_compress.c:149-151)
-				for (u32 k = tid; k < 256 + 259 + 32; k += LZ_THREADS) {
+				for (u32 k = tid; k < 256 + 259 + 32; k += GT) {
 					u32 c;
 					if (k < 256) {
 						c = lens[k] ? lens[k] : 13;
@@ -1424,22 +1384,22 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					}
 					costtab[k] = (u8)c;
 				}
-				__syncthreads();
+				gsync();
 				{
 					const u32 rel_entry = block_entry - block_begin;	// first token of the block
 					const u32 blen_pos = block_end - block_begin;
-					for (u32 seg = warp; seg * LZ_DP_SEG < blen_pos; seg += LZ_WARPS) {
+					for (u32 seg = warp; seg * LZ_DP_SEG < blen_pos; seg += GW) {
 						u32 s0 = seg * LZ_DP_SEG, s1 = s0 + LZ_DP_SEG < blen_pos ? s0 + LZ_DP_SEG : blen_pos;
 						if (s0 < rel_entry) s0 = rel_entry;
 						if (s0 >= s1) continue;
 						lz_dp_segment(ring, mlist, costg, res, costtab, block_begin, s0, s1, lane);
 					}
 				}
-				__syncthreads();
+				gsync();
 				// re-parse the block with the chosen path
-				for (u32 k = tid; k < 320; k += LZ_THREADS) freq[k] = 0;
+				for (u32 k = tid; k < 320; k += GT) freq[k] = 0;
 				if (tid == 0) { v->tok_count = 0; v->parse_entry = block_entry; }
-				__syncthreads();
+				gsync();
 				for (u32 pp = 0; pp < npass_block; pp++) {
 					u32 pb0 = block_begin + pp * LZ_PASS;
 					u32 ppend = pb0 + LZ_PASS < block_end ? pb0 + LZ_PASS : block_end;
@@ -1451,7 +1411,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			// ======================= block flush =========================================
 			LZ_T(7);	// optimal-parse iterations
 			if (tid == 0) freq[256] = 1;
-			__syncthreads();
+			gsync();
 			build_codes();
 			LZ_T(4);	// Huffman codes
 			// (f2) precode items + precode, ref: deflate_compress.c:1483-1631.  Run-length items in
@@ -1472,7 +1432,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				v->hdist = hdist;
 			}
 			if (tid >= 64 && tid < 64 + 19) pfreq_sm[tid - 64] = 0;
-			__syncthreads();
+			gsync();
 			{
 				const u32 hlit = v->hlit, total = hlit + v->hdist;
 				const u32 j = tid;
@@ -1482,7 +1442,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				const bool isstart = inb && val != prv;
 				const u32 smask = __ballot_sync(LDB_FULL_MASK, isstart);
 				if (lane == 0 && warp < 10) escan[66 + warp] = smask;
-				__syncthreads();
+				gsync();
 				u32 run = 0, cnt = 0;
 				if (isstart) {
 					u32 nxt = total;
@@ -1535,7 +1495,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				}
 				if (tid == 0) v->n_items = ntot;
 			}
-			__syncthreads();
+			gsync();
 			if (warp == 0) {
 				// the 19-symbol precode, limited to 7 bits, by warp 0: lane = symbol.  Same construction
 				// as build_codes (rank sort, two-queue merge on lane 0, leaf depths, Kraft repair, lengths
@@ -1612,7 +1572,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					v->extra_bits = 0;
 				}
 			}
-			__syncthreads();
+			gsync();
 			LZ_T(5);	// precode
 			// (f3) symbol costs (ref: deflate_compress.c:1750-1808)
 			if (tid < 320) {
@@ -1631,7 +1591,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					atomicAdd(&v->cost_static, st + extra);
 				}
 			}
-			__syncthreads();
+			gsync();
 			const u32 cost_dyn = v->cost_dyn, cost_static = v->cost_static;
 			// The tokens of this block cover [block_entry, parse_entry): its first token starts where the
 			// previous block's last match ended and its own last match may run past block_end.  A
@@ -1651,17 +1611,17 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			const u64 need_bytes = (o.obit + best + 7) / 8 + (last ? trailer : 0);
 			if (need_bytes > o.avail) {
 				if (tid == 0) v->failed = 1;
-				__syncthreads();
-				break;
+				gsync();
+				return;
 			}
 
 			// staging covers bits starting at word 'w0' of the output; word 0 is seeded with
 			// the partial word carried from the previous flush
 			u64 w0 = o.obit >> 5;
-			for (u32 k = tid; k < LZ_STAGE_WORDS; k += LZ_THREADS) stage[k] = 0;
-			__syncthreads();
+			for (u32 k = tid; k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
+			gsync();
 			if (tid == 0) stage[0] = v->carry;
-			__syncthreads();
+			gsync();
 			if (btype == DEFLATE_BLOCKTYPE_STORED) {
 				// ---- stored: header bits via staging, raw bytes straight from the input
 				u32 src = sbeg;
@@ -1674,22 +1634,22 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 						lz_stage_or(stage, (u32)(ob - (w0 << 5)), (u64)len | ((u64)(~len & 0xffff) << 16), 32);
 					}
 					o.obit = ((o.obit + 3 + 7) & ~(u64)7) + 32;
-					__syncthreads();
+					gsync();
 					// flush staging up to the (byte aligned) current position, byte granular
 					{
 						u64 bytes_end = o.obit >> 3, bytes_begin = w0 * 4;
-						for (u64 k = bytes_begin + tid; k < bytes_end; k += LZ_THREADS) {
+						for (u64 k = bytes_begin + tid; k < bytes_end; k += GT) {
 							u32 rel = (u32)(k - bytes_begin);
 							o.out[k] = (u8)(stage[rel >> 2] >> (8 * (rel & 3)));
 						}
 					}
-					__syncthreads();
-					for (u32 k = tid; k < LZ_STAGE_WORDS; k += LZ_THREADS) stage[k] = 0;
+					gsync();
+					for (u32 k = tid; k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
 					u8 *dst = o.out + (o.obit >> 3);
-					for (u32 k = tid; k < len; k += LZ_THREADS) dst[k] = in[src + k];
+					for (u32 k = tid; k < len; k += GT) dst[k] = in[src + k];
 					src += len;
 					o.obit += (u64)len * 8;
-					__syncthreads();
+					gsync();
 					// re-seed staging word 0 with the bytes already written in the current word
 					w0 = o.obit >> 5;
 					if (tid == 0) {
@@ -1698,16 +1658,16 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 						for (u32 k = 0; k < nb; k++) wv |= (u32)(*(volatile u8 *)(o.out + w0 * 4 + k)) << (8 * k);
 						stage[0] = wv;
 					}
-					__syncthreads();
+					gsync();
 				}
 			} else {
 				// ---- Huffman block --------------------------------------------------------
 				if (btype == DEFLATE_BLOCKTYPE_STATIC) {
-					for (u32 s = tid; s < 320; s += LZ_THREADS) lens[s] = s < 288 ? (u8)lz_static_litlen_len(s) : 5;
-					__syncthreads();
+					for (u32 s = tid; s < 320; s += GT) lens[s] = s < 288 ? (u8)lz_static_litlen_len(s) : 5;
+					gsync();
 					if (tid == 0) lz_gen_codes_serial(lens, 288, codes);
 					if (tid == 32) lz_gen_codes_serial(lens + 288, 32, codes + 288);
-					__syncthreads();
+					gsync();
 				}
 				// header: fixed fields by thread 0, the precode items by one thread each (bit offsets
 				// from a CTA scan), directly into staging
@@ -1741,15 +1701,16 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					}
 					rel = rb;	// bits used in staging so far (relative to word w0)
 				}
-				__syncthreads();
+				gsync();
 				// token rounds: bit lengths -> exclusive scan -> OR into staging -> flush whole words
-				for (u32 t0 = 0; t0 <= ntok; t0 += LZ_EMIT_ROUND) {
+				const u32 tpt = LZ_TPT(GT);
+				for (u32 t0 = 0; t0 <= ntok; t0 += GT * tpt) {
 					// (the EOB symbol is token index ntok)
-					u32 mybits[LZ_TPT] = {};
-					u64 myval[LZ_TPT] = {};
+					u32 mybits[2] = {};
+					u64 myval[2] = {};
 #pragma unroll
-					for (int r = 0; r < LZ_TPT; r++) {
-						u32 ti = t0 + tid * LZ_TPT + r;
+					for (u32 r = 0; r < 2; r++) {
+						u32 ti = r < tpt ? t0 + tid * tpt + r : 0xffffffffu;
 						if (ti < ntok) {
 							u32 tk = tokbuf[ti];
 							if (tk & 0x80000000u) {
@@ -1779,60 +1740,156 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					// CTA-wide exclusive scan of the threads' bit counts
 					u32 mine = 0;
 #pragma unroll
-					for (int r = 0; r < LZ_TPT; r++) mine += mybits[r];
+					for (u32 r = 0; r < 2; r++) mine += mybits[r];
 					u32 incl = mine;
 					for (int o2 = 1; o2 < 32; o2 <<= 1) {
 						u32 t = __shfl_up_sync(LDB_FULL_MASK, incl, o2);
 						if (lane >= (u32)o2) incl += t;
 					}
 					if (lane == 31) escan[warp] = incl;
-					__syncthreads();
+					gsync();
 					if (warp == 0) {
-						u32 x = lane < LZ_WARPS ? escan[lane] : 0;
+						u32 x = lane < GW ? escan[lane] : 0;
 						u32 xi = x;
 						for (int o2 = 1; o2 < 32; o2 <<= 1) {
 							u32 t = __shfl_up_sync(LDB_FULL_MASK, xi, o2);
 							if (lane >= (u32)o2) xi += t;
 						}
-						if (lane < LZ_WARPS) escan[32 + lane] = xi - x;
-						if (lane == LZ_WARPS - 1) escan[64] = xi;
+						if (lane < GW) escan[32 + lane] = xi - x;
+						if (lane == GW - 1) escan[64] = xi;
 					}
-					__syncthreads();
+					gsync();
 					u32 bitpos = rel + escan[32 + warp] + (incl - mine);
 #pragma unroll
-					for (int r = 0; r < LZ_TPT; r++) {
+					for (u32 r = 0; r < 2; r++) {
 						lz_stage_or(stage, bitpos, myval[r], mybits[r]);
 						bitpos += mybits[r];
 					}
 					const u32 round_bits = escan[64];
-					__syncthreads();
+					gsync();
 					rel += round_bits;
 					// flush complete words, keep the partial one as the new stage[0]
 					u32 full = rel >> 5;
 					if (full) {
-						lz_flush_words(o, stage, w0, full);
-						__syncthreads();
+						lz_flush_words(o, stage, w0, full, GT);
+						gsync();
 						u32 carry = stage[full];
-						__syncthreads();
-						for (u32 k = tid; k <= full && k < LZ_STAGE_WORDS; k += LZ_THREADS) stage[k] = 0;
-						__syncthreads();
+						gsync();
+						for (u32 k = tid; k <= full && k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
+						gsync();
 						if (tid == 0) stage[0] = carry;
 						w0 += full;
 						rel &= 31;
-						__syncthreads();
+						gsync();
 					}
 				}
 				o.obit = (w0 << 5) + rel;
 			}
-			__syncthreads();
+			gsync();
 			if (tid == 0) v->carry = stage[0];
 			LZ_T(6);	// costs + emission
 			// ---- next block ------------------------------------------------------------
 			block_begin = block_end;
 			block_entry = v->parse_entry;
-			for (u32 i = tid; i < 320; i += LZ_THREADS) freq[i] = 0;
+			for (u32 i = tid; i < 320; i += GT) freq[i] = 0;
 			if (tid == 0) v->tok_count = 0;
+			gsync();
+		};
+
+		// Pipe: step s loads and inserts pass s (whole CTA); then warps [0, GT) parse pass s - 1 and flush
+		// its block, the others search pass s, and the first group joins that search when it is done.
+		// res[] holds the two passes in flight by parity; the parse's exit table for pass k lives in the
+		// link slots of pass k + 2: insert(k + 1) used them as list scratch and is done with them, and no
+		// chain of pass k + 1 reaches that far back (they belong to positions >= 48 Ki back).
+		const u32 npass = (n + LZ_PASS - 1) / LZ_PASS;
+		for (u32 step = 0; step < npass + (pipe ? 1 : 0); step++) {
+			const u32 b0 = step * LZ_PASS;
+			const u32 pend = b0 + LZ_PASS < n ? b0 + LZ_PASS : n;
+			if (step < npass) {
+				if (tid == 0) v->run_counter = 0;
+				__syncthreads();
+				// (a) window staging by the TMA engine, one pass ahead: searching this pass needs
+				// [b0 - MAX_DIST, pend + LOOKAHEAD), inserting the next one (concurrently) needs the
+				// bytes up to pend + PASS + 3.  The ring then still holds everything back to
+				// b0 - 32768 + 16, i.e. the whole MAX_DIST window.
+				{
+					const u32 want = pend + LZ_PASS + 16 < n ? pend + LZ_PASS + 16 : n;
+					while (loaded_end < want) {
+						u32 room = LZ_RING - (loaded_end & (LZ_RING - 1));	// a segment must not wrap
+						u32 to = loaded_end + (room < LZ_SEG ? room : LZ_SEG);
+						if (to > want) to = want;
+						lz_load_segment(sm, v, in, loaded_end, to);
+						loaded_end = to;
+					}
+				}
+				if (b0 == 0) {
+					// alphabet size of the first 4 KiB -> minimum match length (ref:
+					// calculate_min_match_len, lib/deflate_compress.c:2329-2346)
+					if (tid < 8) { v->used_lits[tid] = 0; v->obs_blk[tid] = 0; }
+					__syncthreads();
+					lz_observe(ring, 0, pend, v->obs_blk, tid, lane, LZ_THREADS);
+					const u32 scan = n < 4096 ? n : 4096;
+					for (u32 i = tid; i < scan; i += LZ_THREADS) {
+						u32 bv = ring[i];
+						atomicOr(&v->used_lits[bv >> 5], 1u << (bv & 31));
+					}
+					__syncthreads();
+					if (tid == 0) {
+						u32 cnt = 0;
+						for (int k = 0; k < 8; k++) cnt += __popc(v->used_lits[k]);
+						v->min_len = n < 512 ? 4 : lz_choose_min_len(cnt, (u32)P.depth);
+						// few distinct byte values = cheap literals (text): a far 4-byte match loses against them
+						v->far4_dist = cnt < 80 ? LZ_FAR4_DIST : LZ_WIN;
+					}
+					__syncthreads();
+				}
+				// (b) the whole CTA links this pass into the hash chains (ordered within a hash)
+				LZ_T(0);	// loads + first-pass extras
+#ifdef LZ_TIMING
+				lz_insert_pass_par(ring, head, nextt, (u32 *)(sm + LZ_SM_R), b0, pend, n, tid, lane, warp, tacc, tlast);
+#else
+				lz_insert_pass_par(ring, head, nextt, (u32 *)(sm + LZ_SM_R), b0, pend, n, tid, lane, warp);
+#endif
+				LZ_T(3);	// insertion: linking
+			}
+			if (!pipe) {
+				// levels 10-12: every position is searched and keeps its list of matches
+				u32 *rs = res + pass_in_block * LZ_PASS;
+				for (u32 i = tid; b0 + i < pend; i += LZ_THREADS) {
+					const u32 p = b0 + i;
+					u32 L = 0, D = 0;
+					u32 *ml = mlist + (size_t)(pass_in_block * LZ_PASS + i) * LZ_OPT_K;
+					if (p + 4 <= n) {
+						lz_search_all(ring, nextt, p, n, P.depth, (u32)P.nice, ml, L, D);
+					} else {
+						for (u32 k = 0; k < LZ_OPT_K; k++) ml[k] = 0;
+					}
+					rs[i] = L ? L | ((D - 1) << 16) : 0;
+				}
+				__syncthreads();
+				LZ_T(1);	// search phase (barrier to barrier)
+				parse_and_flush(b0, pend, pass_in_block * LZ_PASS, nextt + ((b0 + LZ_PASS) & 0xffff));
+			} else {
+				GW = step < npass ? LZ_PWARPS : LZ_WARPS;
+				GT = 32 * GW;
+				if (tid < GT && step) {
+					const u32 kb0 = b0 - LZ_PASS;
+					parse_and_flush(kb0, kb0 + LZ_PASS < n ? kb0 + LZ_PASS : n, ((step - 1) & 1) * LZ_PASS, nextt + ((kb0 + 2 * LZ_PASS) & 0xffff));
+				}
+				if (step < npass) search_pass(b0, pend, res + (step & 1) * LZ_PASS);
+				LZ_T(1);	// search (parse/flush group: its share of the search)
+				if (tid == 0) {
+					v->obit_lo = (u32)o.obit; v->obit_hi = (u32)(o.obit >> 32);
+					v->blk_begin = block_begin; v->blk_entry = block_entry; v->blk_passes = pass_in_block;
+				}
+			}
 			__syncthreads();
+			LZ_T(14);	// wait at the join
+			if (v->failed) break;
+			if (pipe) {	// (every thread takes part in the next whole-CTA parse and flush)
+				o.obit = v->obit_lo | ((u64)v->obit_hi << 32);
+				block_begin = v->blk_begin; block_entry = v->blk_entry; pass_in_block = v->blk_passes;
+			}
 		}
 		__syncthreads();
 		if (v->failed) {
@@ -1866,24 +1923,28 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		LZ_T(7);	// chunk prologue/epilogue
 	}
 #ifdef LZ_TIMING
-	if (tid == 0)
-		for (int k = 0; k < 15; k++) atomicAdd(&ldb_lz_timing[k], (unsigned long long)tacc[k]);
+	if (tid == 0 || tid == 32 * LZ_PWARPS)
+		for (int k = 0; k < 15; k++) atomicAdd(&ldb_lz_timing[tid != 0][k], (unsigned long long)tacc[k]);
 #endif
 }
 
 #ifdef LZ_TIMING
 extern "C" __attribute__((visibility("default"))) void ldb_lz_timing_dump(void)
 {
-	unsigned long long h[16], z[16] = {};
+	unsigned long long h[2][16], z[2][16] = {};
 	cudaDeviceSynchronize();
 	cudaMemcpyFromSymbol(h, ldb_lz_timing, sizeof(h));
 	cudaMemcpyToSymbol(ldb_lz_timing, z, sizeof(z));
-	const char *names[16] = {"loads+first", "search phase", "parse e5", "insert: linking", "huffman", "precode", "cost+emit", "chunk pro/epilogue",
-				 "parse e1", "parse e2", "parse e3", "parse e4", "insert: hashing", "insert: slice lists", "", ""};
-	unsigned long long tot = 0;
-	for (int k = 0; k < 14; k++) tot += h[k];
-	for (int k = 0; k < 16; k++)
-		if (h[k]) printf("  timing %-26s %14llu cycles  %5.1f%%\n", names[k], h[k], 100.0 * (double)h[k] / (double)tot);
+	const char *names[16] = {"loads+first", "search", "parse e5", "insert: linking", "huffman", "precode", "cost+emit", "chunk pro/epilogue",
+				 "parse e1", "parse e2", "parse e3", "parse e4", "insert: hashing", "insert: slice lists", "wait at join", ""};
+	const char *who[2] = {"thread 0 (parse/flush group; levels 10-12: whole CTA)", "first thread of the search group"};
+	for (int g = 0; g < 2; g++) {
+		unsigned long long tot = 0;
+		for (int k = 0; k < 15; k++) tot += h[g][k];
+		printf("  timing, clocked by %s:\n", who[g]);
+		for (int k = 0; k < 16; k++)
+			if (h[g][k]) printf("  timing %-26s %14llu cycles  %5.1f%%\n", names[k], h[g][k], 100.0 * (double)h[g][k] / (double)tot);
+	}
 }
 #endif
 

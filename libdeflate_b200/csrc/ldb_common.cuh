@@ -14,8 +14,30 @@
 #define LDB_LAUNCH(kernel, grid, block, smem, stream, ...) \
 	kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)
 #define LDB_SPIN_PAUSE() __nanosleep(100)
+// barrier 'id' (1..15) over the first 'nthreads' threads that reach it (a multiple of 32)
+#define LDB_BAR_SYNC(id, nthreads) asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory")
 #else
 #define LDB_SPIN_PAUSE() emu::yield()	// cooperative fibers: a spin loop must hand over
+// bar.sync id, nthreads on the emulator's fibers.  All fibers of a block run on one OS thread, one
+// block after the other, so thread-local counters are the block's own; every barrier completes
+// before its block ends, which leaves them at zero for the next block.
+static inline void ldb_emu_bar_sync(unsigned id, unsigned nthreads)
+{
+	static thread_local unsigned arrived[16], gen[16];
+	if (id == 0 || id >= 16 || nthreads == 0 || nthreads % 32 || nthreads > emu::tl_block->nthreads) {
+		fprintf(stderr, "bar.sync %u, %u is not a valid named barrier\n", id, nthreads);
+		abort();
+	}
+	const unsigned mygen = gen[id];
+	if (++arrived[id] == nthreads) {
+		arrived[id] = 0;
+		gen[id]++;
+		emu::tl_block->spins = 0;
+	} else {
+		while (gen[id] == mygen) emu::yield();
+	}
+}
+#define LDB_BAR_SYNC(id, nthreads) ldb_emu_bar_sync((id), (nthreads))
 #endif
 
 typedef uint8_t u8;
