@@ -78,7 +78,7 @@ LIBDEFLATEAPI double libdeflate_b200_timer_stop_ms(struct libdeflate_b200_ctx *c
  * events on the context's stream.  kernel_time_ms() synchronises, then returns the summed
  * duration (ms) and launch count of one kind since the last reset.
  * kind: 0 crc32, 1 adler32, 2 inflate decode (Huffman -> tokens), 3 trailer-verify, 4 deflate,
- *       5 inflate resolve (tokens -> bytes), 6 pack. */
+ *       5 inflate resolve (tokens -> bytes), 6 pack (also the piece setup and stitch of compress_large). */
 LIBDEFLATEAPI void   libdeflate_b200_ctx_set_profiling(struct libdeflate_b200_ctx *ctx, int on);
 LIBDEFLATEAPI double libdeflate_b200_kernel_time_ms(struct libdeflate_b200_ctx *ctx, int kind, uint64_t *n_launches);
 LIBDEFLATEAPI void   libdeflate_b200_kernel_time_reset(struct libdeflate_b200_ctx *ctx);
@@ -210,6 +210,37 @@ libdeflate_b200_bgzf_decompress(struct libdeflate_b200_ctx *ctx,
 				const void *in, size_t in_nbytes,
 				void *out, size_t out_avail,
 				size_t *actual_out, int32_t *result);
+
+/*
+ * One large buffer -> ONE ordinary DEFLATE / zlib / gzip stream (RFC 1951 / 1950 / 1952) that any
+ * inflater reads, compressed by the whole GPU (the pigz method): the input is cut into pieces of
+ * LIBDEFLATE_B200_LARGE_PIECE bytes; piece k is compressed independently with the 32 KiB of input
+ * before it as its dictionary, every piece but the last ends on a byte boundary with an empty stored
+ * block (zlib's sync flush), and the pieces are concatenated behind one header and before one trailer
+ * whose CRC-32 / Adler-32 is combined from the per-piece checksums.  gzip ISIZE is in_nbytes mod 2^32.
+ * For in_nbytes <= LIBDEFLATE_B200_LARGE_PIECE the output is byte-identical to
+ * libdeflate_b200_compress_batch on that one chunk.  The output depends only on (data, level, format).
+ * Unlike libdeflate_b200_bgzf_compress (many gzip members) the result is one stream in every format.
+ *
+ * compress_large: device pointers, asynchronous on the context's stream; *d_out_nbytes (device)
+ *   receives the stream size, or 0 when it did not fit out_avail -- nothing is ever written at or
+ *   beyond d_out + out_avail.  level in [0,12] (-1 = 6).
+ * compress_large_host: host buffers, synchronous, staging included; *out_nbytes is a host size_t.
+ * compress_large_bound: an out_avail that always suffices; for in_nbytes <= the piece size it equals
+ *   libdeflate_{deflate,zlib,gzip}_compress_bound(in_nbytes).
+ * Kernel time of the piece setup and the stitch is reported as kind 6 (pack).
+ */
+#define LIBDEFLATE_B200_LARGE_PIECE  131072   /* input bytes per piece; the output depends on it */
+LIBDEFLATEAPI size_t
+libdeflate_b200_compress_large_bound(int format, size_t in_nbytes);
+LIBDEFLATEAPI int
+libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, int format, int level,
+			       const void *d_in, size_t in_nbytes,
+			       void *d_out, size_t out_avail, size_t *d_out_nbytes);
+LIBDEFLATEAPI int
+libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *ctx, int format, int level,
+				    const void *in, size_t in_nbytes,
+				    void *out, size_t out_avail, size_t *out_nbytes);
 
 #ifdef __cplusplus
 }

@@ -48,7 +48,9 @@ BATCH_SYMBOLS = [
     "libdeflate_b200_decompress_batch_host", "libdeflate_b200_compress_batch_host",
     "libdeflate_b200_decompress_batch_host_packed", "libdeflate_b200_compress_batch_host_packed", "libdeflate_b200_pack_batch",
     "libdeflate_b200_bgzf_compress_bound", "libdeflate_b200_bgzf_compress", "libdeflate_b200_bgzf_decompress",
+    "libdeflate_b200_compress_large_bound", "libdeflate_b200_compress_large", "libdeflate_b200_compress_large_host",
 ]
+LARGE_PIECE = 131072    # LIBDEFLATE_B200_LARGE_PIECE: input bytes per piece of compress_large
 
 
 class Options(ctypes.Structure):
@@ -157,6 +159,12 @@ def load_library(path=None):
     lib.libdeflate_b200_bgzf_compress.argtypes = [P, c_int, P, S, P, S, P]
     lib.libdeflate_b200_bgzf_decompress.restype = c_int
     lib.libdeflate_b200_bgzf_decompress.argtypes = [P, P, S, P, S, P, P]
+    lib.libdeflate_b200_compress_large_bound.restype = S
+    lib.libdeflate_b200_compress_large_bound.argtypes = [c_int, S]
+    lib.libdeflate_b200_compress_large.restype = c_int
+    lib.libdeflate_b200_compress_large.argtypes = [P, c_int, c_int, P, S, P, S, P]
+    lib.libdeflate_b200_compress_large_host.restype = c_int
+    lib.libdeflate_b200_compress_large_host.argtypes = [P, c_int, c_int, P, S, P, S, PS]
     return lib
 
 
@@ -371,6 +379,20 @@ class Context:
             return None
         self._check(rc, "bgzf_compress")
         return out.raw[:n.value]
+
+    def compress_large_bound(self, nbytes, fmt=RAW):
+        return self.l.libdeflate_b200_compress_large_bound(fmt, nbytes)
+
+    def compress_large(self, data, level=6, fmt=RAW, out_avail=None):
+        """One buffer -> ONE raw DEFLATE / zlib / gzip stream compressed by the whole GPU (bytes), or None
+        if out_avail was too small."""
+        addr, n, keep = _buf_ptr(data)
+        avail = self.compress_large_bound(n, fmt) if out_avail is None else out_avail
+        out = ctypes.create_string_buffer(max(avail, 1))
+        r = c_size_t(0)
+        self._check(self.l.libdeflate_b200_compress_large_host(self.h, fmt, level, addr, n, out, avail, ctypes.byref(r)),
+                    "compress_large_host")
+        return ctypes.string_at(out, r.value) if r.value else None
 
     def bgzf_decompress(self, data, out_avail):
         """Blocked gzip file -> (result, bytes or None)."""

@@ -6,50 +6,13 @@
 // lib/gzip_compress.c:32-80, lib/zlib_compress.c:32-72).  Compressed bytes are not
 // contractual (libdeflate.h:76-83) and are NOT the reference's bytes.
 //
-// This file: wrapper header/trailer emission and the stored-block path
+// This file: the stored-block path (wrapper header/trailer writers: ldb_common.cuh)
 // (level 0 and inputs <= 55 - 4*level bytes: ref deflate_compress_none,
 // lib/deflate_compress.c:2393-2443).  The LZ77 + Huffman path is in
 // deflate_lz_kernel.cuh.
 #include "ldb_common.cuh"
 
 #define DEF_THREADS 256
-
-// Writes the wrapper header at out, returns its size (ref: gzip_compress.c:43-62,
-// zlib_compress.c:45-63).
-__device__ __forceinline__ u32 def_write_header(u8 *out, int format, int level)
-{
-	if (format == LDB_FMT_GZIP) {
-		out[0] = 0x1f; out[1] = 0x8b; out[2] = 8; out[3] = 0;
-		out[4] = 0; out[5] = 0; out[6] = 0; out[7] = 0;		// MTIME unavailable
-		out[8] = level < 2 ? 0x04 : (level >= 8 ? 0x02 : 0);	// XFL
-		out[9] = 255;						// OS unknown
-		return 10;
-	}
-	if (format == LDB_FMT_ZLIB) {
-		u32 hint = level < 2 ? 0 : (level < 6 ? 1 : (level < 8 ? 2 : 3));
-		u32 hdr = (8u << 8) | (7u << 12) | (hint << 6);
-		hdr |= 31 - (hdr % 31);
-		out[0] = (u8)(hdr >> 8);
-		out[1] = (u8)hdr;
-		return 2;
-	}
-	return 0;
-}
-
-__device__ __forceinline__ u32 def_write_trailer(u8 *out, int format, u32 checksum, size_t in_nbytes)
-{
-	if (format == LDB_FMT_GZIP) {
-		out[0] = (u8)checksum; out[1] = (u8)(checksum >> 8); out[2] = (u8)(checksum >> 16); out[3] = (u8)(checksum >> 24);
-		u32 isize = (u32)in_nbytes;
-		out[4] = (u8)isize; out[5] = (u8)(isize >> 8); out[6] = (u8)(isize >> 16); out[7] = (u8)(isize >> 24);
-		return 8;
-	}
-	if (format == LDB_FMT_ZLIB) {
-		out[0] = (u8)(checksum >> 24); out[1] = (u8)(checksum >> 16); out[2] = (u8)(checksum >> 8); out[3] = (u8)checksum;
-		return 4;
-	}
-	return 0;
-}
 
 // One CTA per chunk (grid-stride): stored blocks only.
 __global__ void __launch_bounds__(DEF_THREADS)
@@ -71,12 +34,14 @@ ldb_deflate_stored_kernel(ldb_deflate_args a)
 			continue;
 		}
 		if (threadIdx.x == 0) def_write_header(out, a.format, a.level);
+		// a non-final piece of a larger stream: stored blocks end byte-aligned, so no BFINAL is all it needs
+		const bool final_piece = !(a.piece && (a.piece[c] & LDB_PIECE_NONFINAL));
 		u8 *dst = out + hdr;
 		for (size_t b = 0; b < nblocks; b++) {
 			size_t off = b * 65535;
 			u32 len = (u32)(n - off > 65535 ? 65535 : n - off);
 			if (threadIdx.x == 0) {
-				dst[0] = (b + 1 == nblocks) ? 1 : 0;	// BFINAL, BTYPE = 00
+				dst[0] = (b + 1 == nblocks && final_piece) ? 1 : 0;	// BFINAL, BTYPE = 00
 				dst[1] = (u8)len; dst[2] = (u8)(len >> 8);
 				dst[3] = (u8)~len; dst[4] = (u8)(~len >> 8);
 			}

@@ -129,6 +129,7 @@ struct lz_vars {
 	u32 blk_begin, blk_entry, blk_passes;	// block_begin, block_entry, pass_in_block  } every join
 	u32 pre_lens_packed[3];
 	u32 tma_phase;
+	u32 dict, nonfinal;	// the chunk's ldb_deflate_args::piece fields
 };
 
 struct lz_params {
@@ -737,6 +738,11 @@ __device__ __forceinline__ bool lz_should_end_block(const u32 *obs, const u32 *o
 }
 
 // ---- the kernel ----------------------------------------------------------------------------
+// PIECES: the launch carries ldb_deflate_args::piece (pieces of one stream).  The batch path is the
+// instance without it, where the dictionary is 0 and every chunk final at compile time.
+#define LZ_DICT (PIECES ? v->dict : 0u)
+#define LZ_NONFINAL (PIECES && v->nonfinal)
+template <bool PIECES>
 __global__ void __launch_bounds__(LZ_THREADS, 1)
 ldb_deflate_lz_kernel(ldb_deflate_args a)
 {
@@ -806,6 +812,11 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		__syncthreads();
 		if (c >= a.n) break;
 
+		// A piece of a larger stream works in a frame that starts 'dict' bytes before its own input: those
+		// passes are loaded and inserted into the hash chains, never searched, parsed or emitted.
+		const u32 pflags = PIECES ? a.piece[c] : 0;
+		const u32 dict = pflags & LDB_PIECE_DICT_MASK;
+		const bool final_piece = !(pflags & LDB_PIECE_NONFINAL);
 		const u8 *in = (const u8 *)a.in_ptrs[c];
 		const size_t n64 = a.in_nbytes[c];
 		lz_out o;
@@ -832,7 +843,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				size_t off = b * 65535;
 				u32 len = (u32)(n64 - off > 65535 ? 65535 : n64 - off);
 				if (tid == 0) {
-					dst[0] = (b + 1 == nblocks) ? 1 : 0;
+					dst[0] = (b + 1 == nblocks && final_piece) ? 1 : 0;
 					dst[1] = (u8)len; dst[2] = (u8)(len >> 8);
 					dst[3] = (u8)~len; dst[4] = (u8)(~len >> 8);
 				}
@@ -845,13 +856,15 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			}
 			continue;
 		}
-		const u32 n = (u32)n64;
+		const u32 n = (u32)n64 + dict;	// end of the frame
+		in -= dict;
 
 		// ---- per-chunk init ---------------------------------------------------------------
 		for (u32 i = tid; i < (1u << LZ_HASH_BITS) / 2; i += LZ_THREADS) ((u32 *)head)[i] = 0xffffffffu;
 		if (tid == 0) {
 			v->failed = 0;
-			v->parse_entry = 0;
+			v->parse_entry = dict;
+			if (PIECES) { v->dict = dict; v->nonfinal = !final_piece; }
 			v->tok_count = 0;
 			// wrapper header: whole words go straight to the output, the partial word is carried
 			u8 h[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -1220,8 +1233,8 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		};
 
 		u32 loaded_end = 0;
-		u32 block_begin = 0;
-		u32 block_entry = 0;	// position of the first token of the current block
+		u32 block_begin = dict;
+		u32 block_entry = dict;	// position of the first token of the current block
 		u32 pass_in_block = 0;
 
 		// ---- guided search of pass [b0, pend) -> rs[] (levels 1-9; any set of threads, any number of
@@ -1607,8 +1620,9 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			btype = DEFLATE_BLOCKTYPE_STORED;
 			if (cost_static < best) { best = cost_static; btype = DEFLATE_BLOCKTYPE_STATIC; }
 			if (cost_dyn < best) { best = cost_dyn; btype = DEFLATE_BLOCKTYPE_DYNAMIC; }
-			// single bounds check for the whole block (deflate_compress.c:1811-1814)
-			const u64 need_bytes = (o.obit + best + 7) / 8 + (last ? trailer : 0);
+			// single bounds check for the whole block (deflate_compress.c:1811-1814); a non-final piece
+			// ends with an empty stored block: 3 bits, the pad to a byte and 4 bytes, at most 5 bytes
+			const u64 need_bytes = (o.obit + best + 7) / 8 + (last ? (LZ_NONFINAL ? 5 : trailer) : 0);
 			if (need_bytes > o.avail) {
 				if (tid == 0) v->failed = 1;
 				gsync();
@@ -1627,7 +1641,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				u32 src = sbeg;
 				for (u32 piece = 0; piece < stored_pieces; piece++) {
 					u32 len = blen - (src - sbeg) > 65535 ? 65535 : blen - (src - sbeg);
-					bool fin = last && piece + 1 == stored_pieces;
+					bool fin = last && !LZ_NONFINAL && piece + 1 == stored_pieces;
 					if (tid == 0) {
 						lz_stage_or(stage, (u32)(o.obit - (w0 << 5)), fin ? 1 : 0, 3);
 						u64 ob = (o.obit + 3 + 7) & ~(u64)7;
@@ -1675,7 +1689,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				{
 					const u32 rb0 = (u32)(o.obit - (w0 << 5));
 					u32 rb = rb0 + 3;
-					if (tid == 0) lz_stage_or(stage, rb0, (last ? 1 : 0) | (btype << 1), 3);
+					if (tid == 0) lz_stage_or(stage, rb0, (last && !LZ_NONFINAL ? 1 : 0) | (btype << 1), 3);
 					if (btype == DEFLATE_BLOCKTYPE_DYNAMIC) {
 						const u32 hclen = v->hclen, nit = v->n_items;
 						if (tid == 0)
@@ -1801,6 +1815,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		// res[] holds the two passes in flight by parity; the parse's exit table for pass k lives in the
 		// link slots of pass k + 2: insert(k + 1) used them as list scratch and is done with them, and no
 		// chain of pass k + 1 reaches that far back (they belong to positions >= 48 Ki back).
+		// (the passes of the dictionary, step < LZ_DICT / LZ_PASS, are only loaded and inserted)
 		const u32 npass = (n + LZ_PASS - 1) / LZ_PASS;
 		for (u32 step = 0; step < npass + (pipe ? 1 : 0); step++) {
 			const u32 b0 = step * LZ_PASS;
@@ -1822,22 +1837,22 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 						loaded_end = to;
 					}
 				}
-				if (b0 == 0) {
-					// alphabet size of the first 4 KiB -> minimum match length (ref:
-					// calculate_min_match_len, lib/deflate_compress.c:2329-2346)
+				if (b0 == LZ_DICT) {
+					// alphabet size of the first 4 KiB of the chunk's own input -> minimum match length
+					// (ref: calculate_min_match_len, lib/deflate_compress.c:2329-2346)
 					if (tid < 8) { v->used_lits[tid] = 0; v->obs_blk[tid] = 0; }
 					__syncthreads();
-					lz_observe(ring, 0, pend, v->obs_blk, tid, lane, LZ_THREADS);
-					const u32 scan = n < 4096 ? n : 4096;
+					lz_observe(ring, b0, pend, v->obs_blk, tid, lane, LZ_THREADS);
+					const u32 own = n - LZ_DICT, scan = own < 4096 ? own : 4096;
 					for (u32 i = tid; i < scan; i += LZ_THREADS) {
-						u32 bv = ring[i];
+						u32 bv = ring[(b0 + i) & (LZ_RING - 1)];
 						atomicOr(&v->used_lits[bv >> 5], 1u << (bv & 31));
 					}
 					__syncthreads();
 					if (tid == 0) {
 						u32 cnt = 0;
 						for (int k = 0; k < 8; k++) cnt += __popc(v->used_lits[k]);
-						v->min_len = n < 512 ? 4 : lz_choose_min_len(cnt, (u32)P.depth);
+						v->min_len = own < 512 ? 4 : lz_choose_min_len(cnt, (u32)P.depth);
 						// few distinct byte values = cheap literals (text): a far 4-byte match loses against them
 						v->far4_dist = cnt < 80 ? LZ_FAR4_DIST : LZ_WIN;
 					}
@@ -1853,6 +1868,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				LZ_T(3);	// insertion: linking
 			}
 			if (!pipe) {
+				if (PIECES && step < v->dict / LZ_PASS) continue;	// (the insertion ended on a CTA barrier)
 				// levels 10-12: every position is searched and keeps its list of matches
 				u32 *rs = res + pass_in_block * LZ_PASS;
 				for (u32 i = tid; b0 + i < pend; i += LZ_THREADS) {
@@ -1872,11 +1888,11 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			} else {
 				GW = step < npass ? LZ_PWARPS : LZ_WARPS;
 				GT = 32 * GW;
-				if (tid < GT && step) {
+				if (tid < GT && step > LZ_DICT / LZ_PASS) {
 					const u32 kb0 = b0 - LZ_PASS;
 					parse_and_flush(kb0, kb0 + LZ_PASS < n ? kb0 + LZ_PASS : n, ((step - 1) & 1) * LZ_PASS, nextt + ((kb0 + 2 * LZ_PASS) & 0xffff));
 				}
-				if (step < npass) search_pass(b0, pend, res + (step & 1) * LZ_PASS);
+				if (step < npass && (!PIECES || step >= v->dict / LZ_PASS)) search_pass(b0, pend, res + (step & 1) * LZ_PASS);
 				LZ_T(1);	// search (parse/flush group: its share of the search)
 				if (tid == 0) {
 					v->obit_lo = (u32)o.obit; v->obit_hi = (u32)(o.obit >> 32);
@@ -1904,13 +1920,21 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			__syncthreads();
 			if (tid == 0) stage[0] = v->carry;
 			__syncthreads();
-			u64 ob = (o.obit + 7) & ~(u64)7;	// pad the last byte with zero bits
-			if (tid == 0 && trailer) {
-				u8 t[8];
-				def_write_trailer(t, a.format, a.checksums ? a.checksums[c] : 0, n64);
-				for (u32 k = 0; k < trailer; k++) lz_stage_or(stage, (u32)(ob - (w0 << 5)) + 8 * k, t[k], 8);
+			u64 ob;
+			if (!LZ_NONFINAL) {
+				ob = (o.obit + 7) & ~(u64)7;	// pad the last byte with zero bits
+				if (tid == 0 && trailer) {
+					u8 t[8];
+					def_write_trailer(t, a.format, a.checksums ? a.checksums[c] : 0, n64);
+					for (u32 k = 0; k < trailer; k++) lz_stage_or(stage, (u32)(ob - (w0 << 5)) + 8 * k, t[k], 8);
+				}
+				ob += (u64)trailer * 8;
+			} else {
+				// empty stored block (BFINAL 0, BTYPE 00, zero pad, LEN 0000, NLEN FFFF): the piece ends on a byte
+				ob = (o.obit + 3 + 7) & ~(u64)7;
+				if (tid == 0) lz_stage_or(stage, (u32)(ob - (w0 << 5)), 0xffff0000u, 32);
+				ob += 32;
 			}
-			ob += (u64)trailer * 8;
 			__syncthreads();
 			u64 bytes_begin = w0 * 4, bytes_end = ob >> 3;
 			for (u64 k = bytes_begin + tid; k < bytes_end; k += LZ_THREADS) {
@@ -1958,12 +1982,16 @@ size_t ldb_deflate_scratch_bytes(const ldb_launch_cfg &cfg, size_t n)
 static int ldb_launch_deflate_lz(const ldb_deflate_args &a, const ldb_launch_cfg &cfg, void *stream)
 {
 	// per device, cheap: set on every launch (contexts may live on different GPUs and threads)
-	LDB_CUDA_CHECK_RET(cudaFuncSetAttribute(ldb_deflate_lz_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_BYTES));
+	LDB_CUDA_CHECK_RET(cudaFuncSetAttribute(a.piece ? ldb_deflate_lz_kernel<true> : ldb_deflate_lz_kernel<false>,
+						cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_BYTES));
 	ldb_deflate_args b = a;
 	b.work_counter = (u32 *)a.scratch;
 	LDB_CUDA_CHECK_RET(cudaMemsetAsync(b.work_counter, 0, sizeof(u32), (cudaStream_t)stream));
 	size_t blocks = a.n < (size_t)ldb_deflate_grid(cfg) ? a.n : (size_t)ldb_deflate_grid(cfg);
-	LDB_LAUNCH(ldb_deflate_lz_kernel, dim3((unsigned)blocks), dim3(LZ_THREADS), LZ_SM_BYTES, (cudaStream_t)stream, b);
+	if (a.piece)
+		LDB_LAUNCH(ldb_deflate_lz_kernel<true>, dim3((unsigned)blocks), dim3(LZ_THREADS), LZ_SM_BYTES, (cudaStream_t)stream, b);
+	else
+		LDB_LAUNCH(ldb_deflate_lz_kernel<false>, dim3((unsigned)blocks), dim3(LZ_THREADS), LZ_SM_BYTES, (cudaStream_t)stream, b);
 	LDB_CUDA_CHECK_RET(cudaGetLastError());
 	return 0;
 }

@@ -73,6 +73,43 @@ typedef int32_t s32;
 #define DEFLATE_MAX_CODEWORD_LEN   15
 #define DEFLATE_MAX_PRE_CODEWORD_LEN 7
 
+// Writes the wrapper header at out, returns its size (ref: gzip_compress.c:43-62,
+// zlib_compress.c:45-63).  Used by the deflate kernels and by the stream stitch (large_kernels.cu).
+__device__ __forceinline__ u32 def_write_header(u8 *out, int format, int level)
+{
+	if (format == LDB_FMT_GZIP) {
+		out[0] = 0x1f; out[1] = 0x8b; out[2] = 8; out[3] = 0;
+		out[4] = 0; out[5] = 0; out[6] = 0; out[7] = 0;		// MTIME unavailable
+		out[8] = level < 2 ? 0x04 : (level >= 8 ? 0x02 : 0);	// XFL
+		out[9] = 255;						// OS unknown
+		return 10;
+	}
+	if (format == LDB_FMT_ZLIB) {
+		u32 hint = level < 2 ? 0 : (level < 6 ? 1 : (level < 8 ? 2 : 3));
+		u32 hdr = (8u << 8) | (7u << 12) | (hint << 6);
+		hdr |= 31 - (hdr % 31);
+		out[0] = (u8)(hdr >> 8);
+		out[1] = (u8)hdr;
+		return 2;
+	}
+	return 0;
+}
+
+__device__ __forceinline__ u32 def_write_trailer(u8 *out, int format, u32 checksum, size_t in_nbytes)
+{
+	if (format == LDB_FMT_GZIP) {
+		out[0] = (u8)checksum; out[1] = (u8)(checksum >> 8); out[2] = (u8)(checksum >> 16); out[3] = (u8)(checksum >> 24);
+		u32 isize = (u32)in_nbytes;
+		out[4] = (u8)isize; out[5] = (u8)(isize >> 8); out[6] = (u8)(isize >> 16); out[7] = (u8)(isize >> 24);
+		return 8;
+	}
+	if (format == LDB_FMT_ZLIB) {
+		out[0] = (u8)(checksum >> 24); out[1] = (u8)(checksum >> 16); out[2] = (u8)(checksum >> 8); out[3] = (u8)checksum;
+		return 4;
+	}
+	return 0;
+}
+
 // CRC-32 (gzip), reflected generator (ref: lib/crc32.c:51-57)
 #define LDB_CRC32_POLY 0xEDB88320u
 // Adler-32 modulus (ref: lib/adler32.c:31)
@@ -168,10 +205,56 @@ struct ldb_deflate_args {
 	const u32 *checksums;	// per-chunk CRC-32 (gzip) or Adler-32 (zlib) of the input; NULL for raw
 	u8 *scratch;		// per-CTA global scratch (token buffers)
 	u32 *work_counter;	// zero-initialised chunk dispenser
+	// Pieces of one stream (large_kernels.cu); NULL for independent chunks.  piece[c] = the number of
+	// input bytes before in_ptrs[c] that prime the match finder (0 or a multiple of LZ_PASS, at most
+	// 32 KiB) | LDB_PIECE_NONFINAL when the chunk's last block must not be final and the chunk ends
+	// with an empty stored block instead (raw format only).
+	const u32 *piece;
 	size_t n;
 	int format;
 	int level;
 };
+#define LDB_PIECE_NONFINAL 0x80000000u
+#define LDB_PIECE_DICT_MASK 0x7fffffffu
 int ldb_launch_deflate(const ldb_deflate_args &a, const ldb_launch_cfg &cfg, void *stream);
 size_t ldb_deflate_scratch_bytes(const ldb_launch_cfg &cfg, size_t n);
 int ldb_deflate_grid(const ldb_launch_cfg &cfg);
+
+// large_kernels.cu: one buffer -> one stream, cut into pieces of LDB_LARGE_PIECE input bytes (the
+// value of LIBDEFLATE_B200_LARGE_PIECE), processed in waves of consecutive pieces.
+#ifndef LDB_LARGE_PIECE
+#define LDB_LARGE_PIECE 131072
+#endif
+#define LDB_LARGE_DICT 32768	// input bytes before a piece that prime its match finder
+static_assert(LDB_LARGE_PIECE % 16 == 0 && LDB_LARGE_PIECE >= LDB_LARGE_DICT && LDB_LARGE_PIECE <= (1 << 30),
+	      "a piece's dictionary is the input before it");
+// libdeflate_deflate_compress_bound() (ref: lib/deflate_compress.c:4088-4135)
+__host__ __device__ __forceinline__ size_t ldb_raw_bound(size_t n) { return 5 * (n ? (n + 4999) / 5000 : 1) + n; }
+// device slot of one piece: its bound, the closing empty stored block, and 16 bytes the stitch may read past
+#define LDB_LARGE_SLOT ((ldb_raw_bound(LDB_LARGE_PIECE) + 5 + 15) / 16 * 16 + 16)
+struct ldb_large_state {	// carried from wave to wave on the device
+	u64 offset;		// stream bytes of the pieces stitched so far (after the header)
+	u64 sum_len;		// input bytes the running checksum covers
+	u32 sum;		// CRC-32 (gzip) / Adler-32 (zlib) of those bytes
+	u32 failed;		// the stream does not fit (or a piece did not fit its slot)
+};
+struct ldb_large_args {
+	const u8 *in;		// the whole input
+	size_t in_nbytes;
+	u8 *out;		// the stream
+	size_t out_avail;
+	size_t *out_nbytes;	// device: stream size, or 0 -- written by the last wave
+	int format, level;
+	size_t npieces;
+	size_t first, count;	// this wave: pieces [first, first + count)
+	// per piece of the wave
+	const void **in_ptrs;
+	size_t *in_nbytes_k, *out_avail_k, *out_nbytes_k;
+	void **out_ptrs;
+	u32 *piece, *sums;
+	u64 *offsets;
+	u8 *slots;		// piece first + i is compressed into slots + i * LDB_LARGE_SLOT (16-byte aligned)
+	ldb_large_state *state;
+};
+int ldb_launch_large_setup(const ldb_large_args &a, void *stream);
+int ldb_launch_large_stitch(const ldb_large_args &a, void *stream);

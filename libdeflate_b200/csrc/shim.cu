@@ -130,6 +130,7 @@ struct libdeflate_b200_ctx {
 	ldb_buf tmp;			// device: per-batch u32/size_t arrays
 	ldb_buf d_stage_in, d_stage_out;// device staging for host-buffer calls
 	ldb_buf d_pack;			// device: packed output of the *_packed host calls
+	ldb_buf large;			// device: per-wave piece arrays, state and slots of compress_large
 	ldb_buf d_params;		// device: pointer/size arrays for host-buffer calls
 	ldb_buf h_pinned;		// pinned host staging
 	ldb_buf h_pinned_tab;		// pinned host: size / offset tables read back while kernels keep running
@@ -252,6 +253,7 @@ extern "C" void libdeflate_b200_ctx_destroy(struct libdeflate_b200_ctx *ctx)
 	cudaFree(ctx->d_stage_in.p);
 	cudaFree(ctx->d_stage_out.p);
 	cudaFree(ctx->d_pack.p);
+	cudaFree(ctx->large.p);
 	cudaFree(ctx->d_params.p);
 	if (ctx->h_pinned.p) cudaFreeHost(ctx->h_pinned.p);
 	if (ctx->h_pinned_tab.p) cudaFreeHost(ctx->h_pinned_tab.p);
@@ -558,6 +560,7 @@ extern "C" int libdeflate_b200_compress_batch(struct libdeflate_b200_ctx *ctx, i
 	a.checksums = format == LDB_FMT_RAW ? nullptr : sums;
 	a.scratch = (u8 *)ctx->deflate_scratch.p;
 	a.work_counter = nullptr;
+	a.piece = nullptr;
 	a.n = n;
 	a.format = format;
 	a.level = level;
@@ -1066,6 +1069,135 @@ extern "C" int libdeflate_b200_compress_batch_host(struct libdeflate_b200_ctx *c
 		for (size_t i = 0; i < n; i++) h_out_nbytes[i] = r_on[i];
 	}
 	return rc;
+}
+
+// ---------------------------------------------------------------------------------
+// one large buffer -> one stream (large_kernels.cu)
+// ---------------------------------------------------------------------------------
+// Input bytes per wave (default 1 GiB; LIBDEFLATE_B200_LARGE_WAVE_KB overrides): the context keeps the
+// compressed slots of one wave, not of the whole input.  The stream does not depend on it.
+static size_t ldb_large_wave_pieces(void)
+{
+	size_t kb = (size_t)1 << 20;
+	if (const char *e = getenv("LIBDEFLATE_B200_LARGE_WAVE_KB")) {
+		long v = atol(e);
+		if (v > 0) kb = (size_t)v;
+	}
+	const size_t w = (kb << 10) / LDB_LARGE_PIECE;
+	return w ? w : 1;
+}
+
+extern "C" size_t libdeflate_b200_compress_large_bound(int format, size_t in_nbytes)
+{
+	const size_t wrap = format == LDB_FMT_GZIP ? 18 : (format == LDB_FMT_ZLIB ? 6 : 0);
+	if (in_nbytes <= LDB_LARGE_PIECE) return wrap + ldb_raw_bound(in_nbytes);
+	// every piece fits its raw bound; all but the last add their closing empty stored block
+	const size_t full = (in_nbytes - 1) / LDB_LARGE_PIECE;
+	return wrap + full * (ldb_raw_bound(LDB_LARGE_PIECE) + 5) + ldb_raw_bound(in_nbytes - full * LDB_LARGE_PIECE);
+}
+
+extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, int format, int level,
+					       const void *d_in, size_t in_nbytes,
+					       void *d_out, size_t out_avail, size_t *d_out_nbytes)
+{
+	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
+	if (level == -1) level = 6;
+	if (level < 0 || level > 12) return ldb_fail(cudaErrorInvalidValue, "level", __FILE__, __LINE__);
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	const size_t npieces = in_nbytes ? (in_nbytes + LDB_LARGE_PIECE - 1) / LDB_LARGE_PIECE : 1;
+	const size_t wave = npieces < ldb_large_wave_pieces() ? npieces : ldb_large_wave_pieces();
+	// ctx->large: in_ptrs | in_nbytes | out_ptrs | out_avail | out_nbytes | offsets | piece | sums | state | slots
+	const size_t a8 = align_up(wave * 8, 256), a4 = align_up(wave * 4, 256);
+	const size_t slots_off = 6 * a8 + 2 * a4 + 256;
+	int rc = ldb_reserve_dev(ctx->large, slots_off + (npieces > 1 ? wave * LDB_LARGE_SLOT : 0));
+	if (rc) return rc;
+	u8 *b = (u8 *)ctx->large.p;
+	ldb_large_args g;
+	g.in = (const u8 *)d_in;
+	g.in_nbytes = in_nbytes;
+	g.out = (u8 *)d_out;
+	g.out_avail = out_avail;
+	g.out_nbytes = d_out_nbytes;
+	g.format = format;
+	g.level = level;
+	g.npieces = npieces;
+	g.in_ptrs = (const void **)b;
+	g.in_nbytes_k = (size_t *)(b + a8);
+	g.out_ptrs = (void **)(b + 2 * a8);
+	g.out_avail_k = (size_t *)(b + 3 * a8);
+	g.out_nbytes_k = (size_t *)(b + 4 * a8);
+	g.offsets = (u64 *)(b + 5 * a8);
+	g.piece = (u32 *)(b + 6 * a8);
+	g.sums = (u32 *)(b + 6 * a8 + a4);
+	g.state = (ldb_large_state *)(b + 6 * a8 + 2 * a4);
+	g.slots = b + slots_off;
+	if (npieces == 1) {
+		// the whole input is one chunk: exactly what compress_batch makes of it, straight into d_out
+		g.first = 0;
+		g.count = 1;
+		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_setup(g, ctx->stream); });
+		if (rc) return rc;
+		return libdeflate_b200_compress_batch(ctx, format, level, (const void *const *)g.in_ptrs, g.in_nbytes_k,
+						      (void *const *)g.out_ptrs, g.out_avail_k, d_out_nbytes, 1);
+	}
+	rc = ldb_reserve_dev(ctx->deflate_scratch, ldb_deflate_scratch_bytes(ctx->cfg, wave));
+	if (rc) return rc;
+	ldb_deflate_args a;
+	a.in_ptrs = (const void *const *)g.in_ptrs;
+	a.in_nbytes = g.in_nbytes_k;
+	a.out_ptrs = (void *const *)g.out_ptrs;
+	a.out_avail = g.out_avail_k;
+	a.out_nbytes = g.out_nbytes_k;
+	a.checksums = nullptr;		// pieces are raw; the stitch writes the wrapper
+	a.scratch = (u8 *)ctx->deflate_scratch.p;
+	a.work_counter = nullptr;
+	a.piece = g.piece;
+	a.format = LDB_FMT_RAW;
+	a.level = level;
+	for (size_t first = 0; first < npieces; first += wave) {
+		g.first = first;
+		g.count = npieces - first < wave ? npieces - first : wave;
+		a.n = g.count;
+		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_setup(g, ctx->stream); });
+		if (rc) return rc;
+		if (format == LDB_FMT_GZIP)
+			rc = ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, a.in_ptrs, a.in_nbytes, nullptr, g.sums, g.count, ctx->cfg, ctx->stream); });
+		else if (format == LDB_FMT_ZLIB)
+			rc = ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32(a.in_ptrs, a.in_nbytes, nullptr, g.sums, g.count, ctx->cfg, ctx->stream); });
+		if (rc) return rc;
+		rc = ldb_timed_launch(ctx, LDB_K_DEFLATE, [&] { return ldb_launch_deflate(a, ctx->cfg, ctx->stream); });
+		if (rc) return rc;
+		ctx->launches++;	// plan + copy
+		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_stitch(g, ctx->stream); });
+		if (rc) return rc;
+	}
+	return 0;
+}
+
+extern "C" int libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *ctx, int format, int level,
+						    const void *in, size_t in_nbytes,
+						    void *out, size_t out_avail, size_t *out_nbytes)
+{
+	*out_nbytes = 0;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	stream_quiesce quiesce(ctx);
+	int rc = ldb_reserve_dev(ctx->d_stage_in, in_nbytes + 64);
+	if (!rc) rc = ldb_reserve_dev(ctx->d_stage_out, out_avail + 64);
+	if (!rc) rc = ldb_reserve_dev(ctx->d_params, 256);
+	if (rc) return rc;
+	// (the input keeps its 16-byte alignment phase on the device)
+	const u8 *d_in = (const u8 *)ctx->d_stage_in.p + ((uintptr_t)in & 15);
+	size_t *d_res = (size_t *)ctx->d_params.p;
+	if (in_nbytes) LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)d_in, in, in_nbytes, cudaMemcpyHostToDevice, ctx->stream));
+	rc = libdeflate_b200_compress_large(ctx, format, level, d_in, in_nbytes, ctx->d_stage_out.p, out_avail, d_res);
+	if (rc) return rc;
+	size_t r = 0;
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(&r, d_res, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	if (r) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(out, ctx->d_stage_out.p, r, cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	*out_nbytes = r;
+	return 0;
 }
 
 // ---------------------------------------------------------------------------------
