@@ -78,7 +78,8 @@ LIBDEFLATEAPI double libdeflate_b200_timer_stop_ms(struct libdeflate_b200_ctx *c
  * events on the context's stream.  kernel_time_ms() synchronises, then returns the summed
  * duration (ms) and launch count of one kind since the last reset.
  * kind: 0 crc32, 1 adler32, 2 inflate decode (Huffman -> tokens), 3 trailer-verify, 4 deflate,
- *       5 inflate resolve (tokens -> bytes), 6 pack (also the piece setup and stitch of compress_large). */
+ *       5 inflate resolve (tokens -> bytes), 6 pack (also the piece setup and stitch of compress_large, and the
+ *       sync-point scan, window propagation, substitution and results of decompress_large). */
 LIBDEFLATEAPI void   libdeflate_b200_ctx_set_profiling(struct libdeflate_b200_ctx *ctx, int on);
 LIBDEFLATEAPI double libdeflate_b200_kernel_time_ms(struct libdeflate_b200_ctx *ctx, int kind, uint64_t *n_launches);
 LIBDEFLATEAPI void   libdeflate_b200_kernel_time_reset(struct libdeflate_b200_ctx *ctx);
@@ -241,6 +242,44 @@ LIBDEFLATEAPI int
 libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *ctx, int format, int level,
 				    const void *in, size_t in_nbytes,
 				    void *out, size_t out_avail, size_t *out_nbytes);
+
+/*
+ * ONE large DEFLATE / zlib / gzip stream -> its bytes, decoded by the whole GPU where the stream carries
+ * byte-aligned sync points: non-final empty stored blocks (00 00 FF FF), as written after every piece by
+ * libdeflate_b200_compress_large, at every flush by zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH, and between pigz's
+ * blocks.  Segments that start at such points (at least LIBDEFLATE_B200_LARGE_SPLIT_MIN input bytes apart,
+ * default 16384) are decoded at once; a segment is accepted only when the decode from the true stream
+ * start reaches its start, so every result is the serial decode's.  A stream without sync points is one
+ * segment: one decode lane, as libdeflate_b200_decompress_batch would run it.
+ *
+ * Result, actual_in and actual_out are exactly those of libdeflate_{deflate,zlib,gzip}_decompress_ex on
+ * the whole buffer (gzip: the first member; actual_in tells where a next member starts).  Flags as in
+ * decompress_batch (LIBDEFLATE_B200_EXACT_OUT_SIZE).  Output contents are defined on SUCCESS only.
+ * Nothing is written outside [out, out + out_avail), and the input is never written.  All sizes are
+ * size_t: streams above 4 GiB work as long as every segment has less than 4 GiB - 16 bytes of input and
+ * 4 GiB - 32 KiB of output; otherwise the call returns an error code (libdeflate_b200_last_error() says
+ * which) instead of a verdict.
+ *
+ * decompress_large: device pointers.  It WAITS on the context's stream: it reads back the sync-point
+ *   candidates and, per wave of segments, the per-segment results, to plan the chain.  The last kernels
+ *   (checksum, trailer check, results into *d_actual_in, *d_actual_out, *d_result) are queued
+ *   asynchronously.  d_actual_in / d_actual_out may be NULL.
+ * decompress_large_host: host buffers, synchronous, staging included.
+ * decompress_large_segments: the number of segments the last decompress_large on ctx decoded in
+ *   parallel and joined into the stream (1: one lane).
+ * Kernel time: decode as kind 2, resolves as kind 5, the scan, window propagation, substitution and
+ * results as kind 6.
+ */
+LIBDEFLATEAPI int
+libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+				 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
+				 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result);
+LIBDEFLATEAPI int
+libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+				      const void *in, size_t in_nbytes, void *out, size_t out_avail,
+				      size_t *actual_in, size_t *actual_out, int32_t *result);
+LIBDEFLATEAPI size_t
+libdeflate_b200_decompress_large_segments(struct libdeflate_b200_ctx *ctx);
 
 #ifdef __cplusplus
 }

@@ -49,6 +49,7 @@ BATCH_SYMBOLS = [
     "libdeflate_b200_decompress_batch_host_packed", "libdeflate_b200_compress_batch_host_packed", "libdeflate_b200_pack_batch",
     "libdeflate_b200_bgzf_compress_bound", "libdeflate_b200_bgzf_compress", "libdeflate_b200_bgzf_decompress",
     "libdeflate_b200_compress_large_bound", "libdeflate_b200_compress_large", "libdeflate_b200_compress_large_host",
+    "libdeflate_b200_decompress_large", "libdeflate_b200_decompress_large_host", "libdeflate_b200_decompress_large_segments",
 ]
 LARGE_PIECE = 131072    # LIBDEFLATE_B200_LARGE_PIECE: input bytes per piece of compress_large
 
@@ -165,6 +166,12 @@ def load_library(path=None):
     lib.libdeflate_b200_compress_large.argtypes = [P, c_int, c_int, P, S, P, S, P]
     lib.libdeflate_b200_compress_large_host.restype = c_int
     lib.libdeflate_b200_compress_large_host.argtypes = [P, c_int, c_int, P, S, P, S, PS]
+    lib.libdeflate_b200_decompress_large.restype = c_int
+    lib.libdeflate_b200_decompress_large.argtypes = [P, c_int, c_uint, P, S, P, S, P, P, P]
+    lib.libdeflate_b200_decompress_large_host.restype = c_int
+    lib.libdeflate_b200_decompress_large_host.argtypes = [P, c_int, c_uint, P, S, P, S, PS, PS, POINTER(c_int32)]
+    lib.libdeflate_b200_decompress_large_segments.restype = S
+    lib.libdeflate_b200_decompress_large_segments.argtypes = [P]
     return lib
 
 
@@ -393,6 +400,25 @@ class Context:
         self._check(self.l.libdeflate_b200_compress_large_host(self.h, fmt, level, addr, n, out, avail, ctypes.byref(r)),
                     "compress_large_host")
         return ctypes.string_at(out, r.value) if r.value else None
+
+    def decompress_large(self, data, out_avail, fmt=RAW, exact=False):
+        """ONE stream decoded by the whole GPU, split at its sync points (result, bytes or None, actual_in,
+        actual_out) -- the tuple decompress_batch_host gives for the same stream."""
+        addr, n, keep = _buf_ptr(data)
+        out = ctypes.create_string_buffer(max(out_avail, 1))
+        ain = c_size_t(0)
+        aout = c_size_t(0)
+        res = c_int32(0)
+        self._check(self.l.libdeflate_b200_decompress_large_host(
+            self.h, fmt, EXACT_OUT_SIZE if exact else 0, addr, n, out, out_avail,
+            ctypes.byref(ain), ctypes.byref(aout), ctypes.byref(res)), "decompress_large_host")
+        if res.value != SUCCESS:
+            return res.value, None, 0, 0
+        return SUCCESS, ctypes.string_at(out, aout.value), ain.value, aout.value
+
+    def large_segments(self):
+        """Segments the last decompress_large decoded in parallel (1: one lane)."""
+        return self.l.libdeflate_b200_decompress_large_segments(self.h)
 
     def bgzf_decompress(self, data, out_avail):
         """Blocked gzip file -> (result, bytes or None)."""

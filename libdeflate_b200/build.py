@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["shim.cu", "checksum_kernels.cu", "inflate_kernel.cu", "inflate_resolve.cu", "deflate_kernel.cu", "pack_kernels.cu", "large_kernels.cu"]
+SOURCES = ["shim.cu", "checksum_kernels.cu", "inflate_kernel.cu", "inflate_resolve.cu", "deflate_kernel.cu", "pack_kernels.cu", "large_kernels.cu", "large_inflate.cu"]
 HEADERS = ["ldb_common.cuh", "deflate_lz_kernel.cuh"]
 LIB = os.path.join(HERE, "libdeflate_b200.so")
 EMU_DIR = os.path.join(ROOT, "tests", "emu")

@@ -174,6 +174,12 @@ struct inf_lane {
 	// bookkeeping
 	u32 chunk;		// chunk index
 	u32 hdr_bytes;		// wrapper header size
+	// segment mode only (ldb_seg_args): unused, and compiled away, in the batch instance
+	u64 seg_base;		// input offset of 'in' in the whole stream
+	u64 cap;		// slot bytes: tokens that would not fit are counted, not written (inf_seg_fits)
+	u32 reach;		// deepest match reach before the segment start
+	u32 pfx;		// output position of the segment start
+	u32 split_i;		// next split point that a stop may land on
 };
 
 // ---- lane-interleaved table access ------------------------------------------
@@ -703,6 +709,12 @@ extern "C" __attribute__((visibility("default"))) void ldb_inf_stats(unsigned lo
 }
 #endif
 
+// segment mode: may 'extra' more literal bytes and two more records still be written into the slot?
+__device__ __forceinline__ bool inf_seg_fits(const inf_lane &s, u32 extra)
+{
+	return (u64)s.n_lit + extra + 4ull * s.n_rec + 32 <= s.cap;
+}
+
 // ---- decoding: ONE step function for both alphabets -------------------------------------------
 // A lane is either about to read a litlen symbol (ST_LIT) or the offset symbol of a pending length
 // (ST_OFF).  Both are "look up table[bits & mask], maybe a subtable, consume the codeword"; a length
@@ -713,11 +725,15 @@ extern "C" __attribute__((visibility("default"))) void ldb_inf_stats(unsigned lo
 // what counts is the number of instructions per step.
 // The stream ends by moving to ST_DONE with a verdict; the bookkeeping of a finished stream
 // happens once per service phase, outside this loop.
+template <bool SEG>
 __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const u16 *ovf, u32 lane, u32 *wq)
 {
 	// Written as ONE predicated block (selects instead of branches, stores under a predicate, no early
 	// returns): with ~31 of 32 lanes active every path is taken by somebody in every step anyway, so
 	// branches only add reconvergence bookkeeping and register shuttling at the merge points.
+	// Segment mode: a step writes at most 1 + INF_LIT2 literals and two records; once they may not fit
+	// the slot, the step only counts them.
+	const bool wr = !SEG || inf_seg_fits(s, 8);
 	const bool act = s.state >= ST_LIT;
 	const bool isoff = s.state == ST_OFF;
 #if defined(LDB_EMU) && defined(INF_STATS)
@@ -757,7 +773,7 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 	const u32 acc2 = __funnelshift_r(s.acc, e >> 4, 8);
 	s.acc = put ? acc2 : s.acc;
 	s.n_lit += put ? 1u : 0u;
-	if (put && (s.n_lit & 3) == 0) INF_ST_TOK((u32 *)(s.lit + s.n_lit - 4), s.acc);
+	if (wr && put && (s.n_lit & 3) == 0) INF_ST_TOK((u32 *)(s.lit + s.n_lit - 4), s.acc);
 	const u32 vbits = bits >> cl;
 	// length or offset: base(slot) + extra bits, the same arithmetic up to k
 	const u32 slot = (e >> 4) & 31;
@@ -796,10 +812,14 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 	const bool have_off = is_offv || fuse;
 	const bool off_ok = m_off <= inf_out_pos(s);
 	const bool emit = have_off && off_ok;
+	if (SEG && emit) {	// how far before the segment start the match reaches
+		const s32 r = (s32)(m_off + s.pfx - inf_out_pos(s));
+		s.reach = r > (s32)s.reach ? (u32)r : s.reach;
+	}
 	// the match record (and, before it, a literal-run record when more than 255 literals are pending)
 	const u32 litrun = s.n_lit - s.lit_mark;
 	const bool big = litrun > 255;
-	if (emit) {
+	if (wr && emit) {
 		u32 *r = s.rec_end - s.n_rec - 1;
 		if (big) { INF_ST_TOK(r, LDB_TOK_PURE_FLAG | litrun); r--; }
 		INF_ST_TOK(r, ((big ? 0u : litrun) << 23) | ((m_len - 3) << 15) | (m_off - 1));
@@ -826,7 +846,7 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 			const u32 acc3 = __funnelshift_r(s.acc, e2 >> 4, 8);
 			s.acc = more ? acc3 : s.acc;
 			s.n_lit += more ? 1u : 0u;
-			if (more && (s.n_lit & 3) == 0) INF_ST_TOK((u32 *)(s.lit + s.n_lit - 4), s.acc);
+			if (wr && more && (s.n_lit & 3) == 0) INF_ST_TOK((u32 *)(s.lit + s.n_lit - 4), s.acc);
 			adv += more ? (e2 & 15) : 0u;
 			nbits >>= e2 & 15;
 #if defined(LDB_EMU) && defined(INF_STATS)
@@ -899,8 +919,21 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 #ifndef INF_MIN_CTAS
 #define INF_MIN_CTAS 2		// CTAs per SM the register allocation must allow
 #endif
+// Segment mode (SEG, decompress_large): chunk c is a segment of ONE stream, described by g (ldb_common.cuh).
+// The batch instance (SEG = false) compiles to the code it had before the mode existed.
+
+// a non-final empty stored block has ended at byte 'next' of the segment: is that a split point at or
+// after the segment's next one?  (The index passes split points that lie before the block end.)
+__device__ __forceinline__ bool inf_seg_stop(inf_lane &s, const ldb_seg_args &g, u32 next)
+{
+	const u64 e = s.seg_base + next;
+	while (s.split_i < g.nsplit && g.split[s.split_i] < e) s.split_i++;
+	return s.split_i < g.nsplit && g.split[s.split_i] == e;
+}
+
+template <bool SEG>
 __global__ void __launch_bounds__(32 * INF_WPC, INF_MIN_CTAS)
-ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)
+ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 {
 	LDB_DYN_SMEM(sm_cta);
 	u8 *sm = sm_cta + (threadIdx.x >> 5) * INF_SM_BYTES;
@@ -921,6 +954,46 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)
 	// the bookkeeping of a stream that has ended (ST_DONE) with s.verdict; the lane becomes idle
 	auto finish = [&]() {
 		const size_t c = s.chunk;
+		if constexpr (SEG) {
+			ldb_seg_info r;
+			u32 verdict = s.verdict;
+			const u64 P = inf_bits_consumed(s);
+			r.end = 0; r.trailer = 0; r.isize = 0; r.pad = 0; r.overflow = 0;
+			r.split_j = s.split_i;
+			if (verdict == LDB_SUCCESS) {
+				if (P > (u64)s.in_n * 8) verdict = LDB_BAD_DATA;	// decompress_template.h:754
+				else {
+					const u32 used = (u32)((P + 7) >> 3);
+					const u8 *t = s.in + used;	// the trailer (the segment's input ends before it)
+					r.end = s.seg_base + used;
+					if (a.format == LDB_FMT_GZIP) {
+						r.trailer = t[0] | ((u32)t[1] << 8) | ((u32)t[2] << 16) | ((u32)t[3] << 24);
+						r.isize = t[4] | ((u32)t[5] << 8) | ((u32)t[6] << 16) | ((u32)t[7] << 24);
+					} else if (a.format == LDB_FMT_ZLIB) {
+						r.trailer = ((u32)t[0] << 24) | ((u32)t[1] << 16) | ((u32)t[2] << 8) | t[3];
+					}
+				}
+			} else if (verdict == LDB_SEG_STOPPED) {
+				r.end = s.seg_base + (P >> 3);
+			}
+			if (verdict == LDB_SUCCESS || verdict == LDB_SEG_STOPPED) {
+				const bool fits = inf_seg_fits(s, 8);
+				if (fits) inf_flush_pending(s);
+				if (s.n_lit != s.lit_mark) {
+					if (fits) inf_put_record(s, LDB_TOK_PURE_FLAG | (s.n_lit - s.lit_mark));
+					else s.n_rec++;
+				}
+				r.overflow = !fits;
+			}
+			r.verdict = verdict;
+			r.out_len = inf_out_pos(s) - s.pfx;
+			r.reach = s.reach;
+			r.n_rec = s.n_rec;
+			r.n_lit = s.n_lit;
+			g.info[c] = r;
+			s.state = ST_IDLE;
+			return;
+		}
 		int verdict = (int)s.verdict;
 		const u32 out_pos = inf_out_pos(s);
 		u32 footer = a.format == LDB_FMT_GZIP ? 8 : (a.format == LDB_FMT_ZLIB ? 4 : 0);
@@ -979,6 +1052,49 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)
 					} else {
 						c += a.first;
 						s.chunk = (u32)c;
+						if constexpr (SEG) {
+							const u64 st = g.start[c];
+							const u32 pfx = g.pfx[c];
+							const size_t oa = a.out_avail[c];
+							s.out_avail = oa > 0xfffffff0u - pfx ? 0xfffffff0u : (u32)oa + pfx;
+							s.lit_limit = s.out_avail;
+							s.acc = 0;
+							s.pend_len = 0;
+							s.lit = a.tok_base + (a.tok_off[c] - a.tok_origin);
+							s.rec_end = (u32 *)(a.tok_base + (a.tok_off[c + 1] - a.tok_origin));
+							s.cap = a.tok_off[c + 1] - a.tok_off[c];
+							s.n_lit = pfx;		// the prefix: output positions before the segment start
+							s.n_rec = 0;
+							s.lit_mark = 0;
+							s.pfx = pfx;
+							s.reach = 0;
+							s.split_i = g.split_i[c];
+							u32 footer = a.format == LDB_FMT_GZIP ? 8 : (a.format == LDB_FMT_ZLIB ? 4 : 0);
+							u64 skip = st;
+							if (st == 0) {	// the stream start: the wrapper header is parsed here only
+								const u32 hdr = inf_parse_wrapper(g.base, g.in_nbytes, a.format, &footer);
+								skip = hdr == 0xffffffffu ? ~(u64)0 : hdr;
+							}
+							if (skip == ~(u64)0) {
+								s.verdict = LDB_BAD_DATA;
+								s.state = ST_DONE;
+								s.in = g.base;
+								s.seg_base = 0;
+								s.in_n = 0;
+								s.in_a0 = 0; s.in_al = g.base; s.in_nal = 0; s.wpos = 0; s.bitpos = 0;
+							} else {
+								const u64 dn = g.in_nbytes - footer - skip;
+								s.in = g.base + skip;
+								s.seg_base = skip;
+								s.in_n = dn > 0xfffffff0u ? 0xfffffff0u : (u32)dn;
+								s.in_a0 = (u32)(uintptr_t)s.in & 3;
+								s.in_al = s.in - s.in_a0;
+								s.in_nal = s.in_a0 + s.in_n;
+								s.hdr_bytes = 0;
+								inf_bits_init(s, 0);
+								s.state = ST_HEADER;
+							}
+						} else {
 						const u8 *in = (const u8 *)a.in_ptrs[c];
 						size_t n = a.in_nbytes[c];
 						size_t oa = a.out_avail[c];
@@ -1009,6 +1125,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)
 							inf_bits_init(s, 0);
 							s.state = ST_HEADER;
 						}
+						}
 					}
 				}
 			}
@@ -1027,19 +1144,25 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)
 				u32 owner = __ffs(stored) - 1;
 				stored &= stored - 1;
 				// the owner's pending literal bytes must be in memory first
-				if (lane == owner) inf_flush_pending(s);
+				// (segment mode: a block that may not fit the slot is counted, not copied)
+				const bool cp = !SEG || inf_seg_fits(s, s.stored_len + 8);
+				if (lane == owner && cp) inf_flush_pending(s);
 				__syncwarp();
 				const u8 *src = (const u8 *)__shfl_sync(LDB_FULL_MASK, (u64)(uintptr_t)(s.in + s.stored_src), owner);
 				u8 *dst = (u8 *)__shfl_sync(LDB_FULL_MASK, (u64)(uintptr_t)(s.lit + s.n_lit), owner);
 				u32 len = __shfl_sync(LDB_FULL_MASK, s.stored_len, owner);
+				if (SEG) len = __shfl_sync(LDB_FULL_MASK, cp ? len : 0u, owner);
 				inf_warp_copy(dst, src, len, lane);
 				__syncwarp();
 				if (lane == owner) {
+					if (SEG) len = s.stored_len;
 					s.n_lit += len;
-					inf_reload_pending(s);
+					if (!SEG || inf_seg_fits(s, 8)) inf_reload_pending(s);
+					else s.acc = 0;
 					u32 next = s.stored_src + len;
 					inf_bits_init(s, next);	// P = 8 * next exactly
 					if (s.is_final) { s.verdict = LDB_SUCCESS; s.state = ST_DONE; }
+					else if (SEG && len == 0 && inf_seg_stop(s, g, next)) { s.verdict = LDB_SEG_STOPPED; s.state = ST_DONE; }
 					else s.state = ST_HEADER;	// parsed in the next repetition
 				}
 			}
@@ -1087,7 +1210,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter)
 		*(volatile u32 *)(wq + 32) = s.state >= ST_LIT ? inf_ld_word(s, s.wpos + 12) : 0;
 #endif
 		for (int it = 0; it < INF_QUANTUM; it++) {
-			inf_decode_step(s, sm, ovf, lane, wq);
+			inf_decode_step<SEG>(s, sm, ovf, lane, wq);
 			if ((it & 31) == 31 && !__any_sync(LDB_FULL_MASK, s.state >= ST_LIT)) break;
 		}
 		inf_cp_async_wait();
@@ -1116,19 +1239,31 @@ __global__ void ldb_verify_trailer_kernel(ldb_inflate_args a, const u32 *checksu
 		a.results[c] = LDB_BAD_DATA;
 }
 
-int ldb_launch_inflate(const ldb_inflate_args &a, const ldb_launch_cfg &cfg, void *stream)
+template <bool SEG>
+static int inf_launch(const ldb_inflate_args &a, const ldb_seg_args &g, const ldb_launch_cfg &cfg, void *stream)
 {
 	if (a.count == 0) return 0;
 	// the attribute is per device and cheap to set: every launch does it (a context may live on any GPU)
-	LDB_CUDA_CHECK_RET(cudaFuncSetAttribute(ldb_inflate_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, INF_WPC * INF_SM_BYTES));
+	LDB_CUDA_CHECK_RET(cudaFuncSetAttribute(ldb_inflate_decode_kernel<SEG>, cudaFuncAttributeMaxDynamicSharedMemorySize, INF_WPC * INF_SM_BYTES));
 	u32 *counter = (u32 *)a.overflow_scratch;	// the first 256 bytes of the scratch hold the two work counters
 	LDB_CUDA_CHECK_RET(cudaMemsetAsync(counter, 0, 2 * sizeof(u32), (cudaStream_t)stream));
 	size_t blocks = (a.count + 32 * INF_WPC - 1) / (32 * INF_WPC);
 	size_t cap = (size_t)ldb_inflate_grid_blocks(cfg) / INF_WPC;
 	if (blocks > cap) blocks = cap;
-	LDB_LAUNCH(ldb_inflate_decode_kernel, dim3((unsigned)blocks), dim3(32 * INF_WPC), INF_WPC * INF_SM_BYTES, (cudaStream_t)stream, a, counter);
+	LDB_LAUNCH(ldb_inflate_decode_kernel<SEG>, dim3((unsigned)blocks), dim3(32 * INF_WPC), INF_WPC * INF_SM_BYTES, (cudaStream_t)stream, a, counter, g);
 	LDB_CUDA_CHECK_RET(cudaGetLastError());
 	return 0;
+}
+
+int ldb_launch_inflate(const ldb_inflate_args &a, const ldb_launch_cfg &cfg, void *stream)
+{
+	ldb_seg_args none = {};
+	return inf_launch<false>(a, none, cfg, stream);
+}
+
+int ldb_launch_inflate_seg(const ldb_inflate_args &a, const ldb_seg_args &g, const ldb_launch_cfg &cfg, void *stream)
+{
+	return inf_launch<true>(a, g, cfg, stream);
 }
 
 // work counter of the resolve kernel (zeroed by ldb_launch_inflate together with the decoder's)

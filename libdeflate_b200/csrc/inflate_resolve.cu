@@ -198,8 +198,12 @@ __device__ __forceinline__ void res_copy_coop(const u8 *win, u8 *stg, u32 B, u32
 }
 
 // ---- the kernel ----------------------------------------------------------------------------------
+// ALT_LIT (decompress_large): every chunk takes its literal bytes from 'alt_lit' instead of the front of
+// its slot -- the records alone are walked again, over other bytes.  That is how the high byte plane of
+// 16-bit symbols is resolved (large_inflate.cu).  The batch instance (ALT_LIT = false) is unchanged.
+template <bool ALT_LIT>
 __global__ void __launch_bounds__(32, RES_PER_SM)
-ldb_inflate_resolve_kernel(ldb_inflate_args a, u32 *work_counter)
+ldb_inflate_resolve_kernel(ldb_inflate_args a, u32 *work_counter, const u8 *alt_lit)
 {
 	LDB_DYN_SMEM(sm);
 	u8 *stg = sm;
@@ -213,7 +217,7 @@ ldb_inflate_resolve_kernel(ldb_inflate_args a, u32 *work_counter)
 		const size_t c = a.first + idx;
 		const u32 n_rec = a.tok_counts[2 * c];
 		if (n_rec == 0) continue;
-		const u8 *lit = a.tok_base + (a.tok_off[c] - a.tok_origin);
+		const u8 *lit = ALT_LIT ? alt_lit : a.tok_base + (a.tok_off[c] - a.tok_origin);
 		const u32 *rec_end = (const u32 *)(a.tok_base + (a.tok_off[c + 1] - a.tok_origin));
 		u8 *const out = (u8 *)a.out_ptrs[c];
 		// shifted coordinates: q = output position + a0, so that q % 16 is the alignment phase of the
@@ -326,17 +330,28 @@ ldb_inflate_resolve_kernel(ldb_inflate_args a, u32 *work_counter)
 	}
 }
 
-int ldb_launch_inflate_resolve(const ldb_inflate_args &a, const ldb_launch_cfg &cfg, void *stream)
+template <bool ALT_LIT>
+static int res_launch(const ldb_inflate_args &a, const u8 *alt_lit, const ldb_launch_cfg &cfg, void *stream)
 {
 	if (a.count == 0) return 0;
 	u32 *d_counter = ldb_inflate_resolve_counter(a, cfg);
-	LDB_CUDA_CHECK_RET(cudaFuncSetAttribute(ldb_inflate_resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RES_SM_BYTES));
+	LDB_CUDA_CHECK_RET(cudaFuncSetAttribute(ldb_inflate_resolve_kernel<ALT_LIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, RES_SM_BYTES));
 	int per_sm = (cfg.max_smem_optin + 1024) / (RES_SM_BYTES + 1024);
 	if (per_sm < 1) per_sm = 1;
 	if (per_sm > RES_PER_SM) per_sm = RES_PER_SM;
 	size_t blocks = (size_t)cfg.num_sms * per_sm;
 	if (blocks > a.count) blocks = a.count;
-	LDB_LAUNCH(ldb_inflate_resolve_kernel, dim3((unsigned)blocks), dim3(32), RES_SM_BYTES, (cudaStream_t)stream, a, d_counter);
+	LDB_LAUNCH(ldb_inflate_resolve_kernel<ALT_LIT>, dim3((unsigned)blocks), dim3(32), RES_SM_BYTES, (cudaStream_t)stream, a, d_counter, alt_lit);
 	LDB_CUDA_CHECK_RET(cudaGetLastError());
 	return 0;
+}
+
+int ldb_launch_inflate_resolve(const ldb_inflate_args &a, const ldb_launch_cfg &cfg, void *stream)
+{
+	return res_launch<false>(a, nullptr, cfg, stream);
+}
+
+int ldb_launch_inflate_resolve_lit(const ldb_inflate_args &a, const u8 *lit, const ldb_launch_cfg &cfg, void *stream)
+{
+	return res_launch<true>(a, lit, cfg, stream);
 }

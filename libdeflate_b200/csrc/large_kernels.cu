@@ -45,41 +45,6 @@ ldb_large_setup_kernel(ldb_large_args a)
 	}
 }
 
-// ---- checksum combine ------------------------------------------------------------------------------
-// CRC-32 (reflected): a * b mod G; x^(8 * 2^i) mod G in xp[i]
-__device__ __forceinline__ u32 lg_mulmodp(u32 a, u32 b)
-{
-	u32 p = 0;
-	for (int i = 0; i < 32; i++) {
-		if (a & 0x80000000u) p ^= b;
-		a <<= 1;
-		b = (b >> 1) ^ ((b & 1) ? LDB_CRC32_POLY : 0);
-	}
-	return p;
-}
-
-// checksum of A || B from those of A and B (len_b = |B|): CRC-32 is linear, crc(A || B) =
-// crc(A) * x^(8 len_b) + crc(B); Adler-32 by the zlib rule.  (init, 0) is the identity on both sides.
-__device__ __forceinline__ u32 lg_combine(int format, const u32 *xp, u32 a, u32 b, u64 len_b)
-{
-	if (format == LDB_FMT_GZIP) {
-		u32 m = 0x80000000u;	// x^0
-		for (int i = 0; len_b; i++, len_b >>= 1)
-			if (len_b & 1) m = lg_mulmodp(xp[i], m);
-		return lg_mulmodp(m, a) ^ b;
-	}
-	const u32 M = LDB_ADLER_MOD;
-	const u32 rem = (u32)(len_b % M);
-	u32 s1 = a & 0xffff, s2 = (u32)(((u64)rem * s1) % M);
-	s1 += (b & 0xffff) + M - 1;
-	s2 += (a >> 16) + (b >> 16) + M - rem;
-	if (s1 >= M) s1 -= M;
-	if (s1 >= M) s1 -= M;
-	if (s2 >= (M << 1)) s2 -= (M << 1);
-	if (s2 >= M) s2 -= M;
-	return s1 | (s2 << 16);
-}
-
 #define LG_PLAN_THREADS 1024
 // One CTA.  Thread t owns a contiguous range of the wave's pieces: it sums their sizes and folds their
 // checksums in order; a CTA scan of the sizes gives every piece its offset, a tree of ordered combines
@@ -97,7 +62,7 @@ ldb_large_plan_kernel(ldb_large_args a)
 	if (tid == 0) {
 		any_empty = 0;
 		u32 x = 0x00800000u;	// x^8
-		for (int i = 0; i < 64; i++) { xp[i] = x; x = lg_mulmodp(x, x); }
+		for (int i = 0; i < 64; i++) { xp[i] = x; x = ldb_mulmodp(x, x); }
 	}
 	__syncthreads();
 	const size_t per = (a.count + LG_PLAN_THREADS - 1) / LG_PLAN_THREADS;
@@ -111,7 +76,7 @@ ldb_large_plan_kernel(ldb_large_args a)
 		empty |= sz == 0;	// a piece that did not fit its slot (cannot happen: the slots hold the bound)
 		bytes += sz;
 		if (ck) {
-			sum = lg_combine(a.format, xp, sum, a.sums[i], a.in_nbytes_k[i]);
+			sum = ldb_sum_combine(a.format, xp, sum, a.sums[i], a.in_nbytes_k[i]);
 			len += a.in_nbytes_k[i];
 		}
 	}
@@ -136,7 +101,7 @@ ldb_large_plan_kernel(ldb_large_args a)
 	// ordered tree of the per-thread checksums: node tid covers threads [tid, tid + 2s)
 	for (u32 s = 1; s < LG_PLAN_THREADS; s <<= 1) {
 		if (ck && (tid & (2 * s - 1)) == 0) {
-			tv[tid] = lg_combine(a.format, xp, tv[tid], tv[tid + s], tl[tid + s]);
+			tv[tid] = ldb_sum_combine(a.format, xp, tv[tid], tv[tid + s], tl[tid + s]);
 			tl[tid] += tl[tid + s];
 		}
 		__syncthreads();
@@ -146,7 +111,7 @@ ldb_large_plan_kernel(ldb_large_args a)
 		const bool last = a.first + a.count == a.npieces;
 		const u64 total = pos;
 		const u32 failed = st.failed || any_empty || (u64)hdr + total + (last ? trl : 0) > a.out_avail;
-		const u32 run = ck ? lg_combine(a.format, xp, st.sum, tv[0], tl[0]) : 0;
+		const u32 run = ck ? ldb_sum_combine(a.format, xp, st.sum, tv[0], tl[0]) : 0;
 		if (!failed && a.first == 0) def_write_header(a.out, a.format, a.level);
 		if (last) {
 			if (!failed) def_write_trailer(a.out + hdr + total, a.format, run, a.in_nbytes);

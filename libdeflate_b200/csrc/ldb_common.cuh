@@ -115,6 +115,42 @@ __device__ __forceinline__ u32 def_write_trailer(u8 *out, int format, u32 checks
 // Adler-32 modulus (ref: lib/adler32.c:31)
 #define LDB_ADLER_MOD  65521u
 
+// ---- checksum combine (compress_large's stitch, decompress_large's trailer check) -------------------
+// CRC-32 (reflected): a * b mod G
+__device__ __forceinline__ u32 ldb_mulmodp(u32 a, u32 b)
+{
+	u32 p = 0;
+	for (int i = 0; i < 32; i++) {
+		if (a & 0x80000000u) p ^= b;
+		a <<= 1;
+		b = (b >> 1) ^ ((b & 1) ? LDB_CRC32_POLY : 0);
+	}
+	return p;
+}
+
+// checksum of A || B from those of A and B (len_b = |B|): CRC-32 is linear, crc(A || B) =
+// crc(A) * x^(8 len_b) + crc(B), with x^(8 * 2^i) mod G in xp[i]; Adler-32 by the zlib rule.
+// (init, 0) is the identity on both sides.
+__device__ __forceinline__ u32 ldb_sum_combine(int format, const u32 *xp, u32 a, u32 b, u64 len_b)
+{
+	if (format == LDB_FMT_GZIP) {
+		u32 m = 0x80000000u;	// x^0
+		for (int i = 0; len_b; i++, len_b >>= 1)
+			if (len_b & 1) m = ldb_mulmodp(xp[i], m);
+		return ldb_mulmodp(m, a) ^ b;
+	}
+	const u32 M = LDB_ADLER_MOD;
+	const u32 rem = (u32)(len_b % M);
+	u32 s1 = a & 0xffff, s2 = (u32)(((u64)rem * s1) % M);
+	s1 += (b & 0xffff) + M - 1;
+	s2 += (a >> 16) + (b >> 16) + M - rem;
+	if (s1 >= M) s1 -= M;
+	if (s1 >= M) s1 -= M;
+	if (s2 >= (M << 1)) s2 -= (M << 1);
+	if (s2 >= M) s2 -= M;
+	return s1 | (s2 << 16);
+}
+
 // Constant tables for the checksum kernels, computed once on the host by the
 // shim (ldb_build_crc_tables) and kept in device memory per context.
 struct ldb_crc_tables {
@@ -191,6 +227,60 @@ size_t ldb_inflate_overflow_bytes_per_stream(void);
 int ldb_inflate_grid_blocks(const ldb_launch_cfg &cfg);
 size_t ldb_inflate_scratch_bytes(const ldb_launch_cfg &cfg, size_t n);
 int ldb_launch_verify_trailer(const ldb_inflate_args &a, const u32 *d_checksums, void *stream);
+
+// ---- segment mode of the decode kernel (decompress_large, DESIGN.md section 4.6) ----------------------
+// Chunk c of the launch is a SEGMENT of one stream: it starts at byte start[c] of the whole input (0: the
+// stream start, wrapper header parsed there) and its input runs to the end of the DEFLATE data.  Its
+// output position starts at pfx[c] (matches may reach that far before the segment), the literal stream
+// keeps pfx[c] bytes free at the front of the slot, and out_avail[c] is the room after the prefix.  The
+// lane stops after a non-final empty stored block that ends on one of the sorted split points
+// split[j], j >= split_i[c].  Tokens that do not fit the slot are counted, not written.
+#define LDB_SEG_PREFIX 32768u
+struct ldb_seg_info {
+	u64 end;		// input offset after the segment (stop: a split point; final block: after its last byte)
+	u32 verdict;		// LDB_* result, or LDB_SEG_STOPPED
+	u32 out_len;		// output bytes (the prefix not counted)
+	u32 reach;		// deepest match reach before the segment start (0: none)
+	u32 split_j;		// stop: index of the split point it stopped at
+	u32 n_rec, n_lit;	// token counts (n_lit includes the prefix)
+	u32 overflow;		// the tokens did not fit the slot (counts are exact, contents incomplete)
+	u32 trailer, isize;	// final block: the trailer fields that follow it
+	u32 pad;
+};
+#define LDB_SEG_STOPPED 16
+struct ldb_seg_args {
+	const u8 *base;		// the whole input
+	u64 in_nbytes;
+	const u64 *split;	// chosen split points, ascending
+	u32 nsplit;
+	const u64 *start;	// per chunk
+	const u32 *pfx;
+	const u32 *split_i;
+	ldb_seg_info *info;
+};
+int ldb_launch_inflate_seg(const ldb_inflate_args &a, const ldb_seg_args &g, const ldb_launch_cfg &cfg, void *stream);
+// resolve of the high byte plane of 16-bit symbols: every chunk reads its literals from 'lit' instead of its slot
+int ldb_launch_inflate_resolve_lit(const ldb_inflate_args &a, const u8 *lit, const ldb_launch_cfg &cfg, void *stream);
+
+// large_inflate.cu
+struct ldb_chain_seg {		// one segment of the decode chain, as the propagation and substitution see it
+	const u8 *lo, *hi;	// symbol planes at the segment start (hi NULL: every symbol is the byte in lo)
+	u8 *dst;		// out + G_k, or NULL when lo already is the output
+	u64 len;
+};
+int ldb_launch_sync_scan_count(const u8 *in, size_t n, u32 *d_counts, size_t tiles, void *stream);
+int ldb_launch_sync_scan_write(const u8 *in, size_t n, const u64 *d_tile_off, u64 *d_cand, size_t tiles, void *stream);
+size_t ldb_sync_scan_tiles(size_t n);
+int ldb_launch_seg_prefix_fill(u8 *const *d_lit, size_t n, void *stream);
+int ldb_launch_window_chain(const ldb_chain_seg *d_segs, size_t n, u8 *d_windows, void *stream);
+int ldb_launch_substitute(const ldb_chain_seg *d_segs, size_t n, const u8 *d_windows, void *stream);
+struct ldb_large_verdict {
+	s32 result;		// decided on the host; SUCCESS may still turn into BAD_DATA at the trailer check
+	u32 trailer, isize;
+	u64 actual_in, actual_out;
+};
+int ldb_launch_large_inflate_finish(const u32 *d_sums, const size_t *d_lens, size_t n, int format, const ldb_large_verdict &v,
+				    size_t *d_actual_in, size_t *d_actual_out, s32 *d_result, void *stream);
 
 // pack_kernels.cu: chunk i -> d_dense + d_offsets[i], offsets = prefix sums of the sizes rounded up to 16
 int ldb_launch_pack(const void *const *d_ptrs, const size_t *d_sizes, size_t n, void *d_dense, size_t dense_avail,

@@ -14,6 +14,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <vector>
 
 #include "../../include/libdeflate.h"
@@ -131,6 +132,10 @@ struct libdeflate_b200_ctx {
 	ldb_buf d_stage_in, d_stage_out;// device staging for host-buffer calls
 	ldb_buf d_pack;			// device: packed output of the *_packed host calls
 	ldb_buf large;			// device: per-wave piece arrays, state and slots of compress_large
+	// decompress_large (device): sync-point scan + split list, per-wave arrays, re-decoded tokens,
+	// symbol planes, windows, the carried window, the high-plane literal stream, checksum arrays
+	ldb_buf li_scan, li_arr, li_tok2, li_planes, li_win, li_carry, li_hilit, li_sums;
+	size_t li_segments;		// chain segments of the last decompress_large
 	ldb_buf d_params;		// device: pointer/size arrays for host-buffer calls
 	ldb_buf h_pinned;		// pinned host staging
 	ldb_buf h_pinned_tab;		// pinned host: size / offset tables read back while kernels keep running
@@ -213,6 +218,7 @@ extern "C" struct libdeflate_b200_ctx *libdeflate_b200_ctx_create(int device)
 	ctx->ev_stop = nullptr;
 	ctx->stream_h2d = nullptr;
 	ctx->stream_d2h = nullptr;
+	ctx->li_segments = 0;
 	cudaStreamCreateWithFlags(&ctx->stream_h2d, cudaStreamNonBlocking);
 	cudaStreamCreateWithFlags(&ctx->stream_d2h, cudaStreamNonBlocking);
 	cudaEventCreate(&ctx->ev_start);
@@ -254,6 +260,8 @@ extern "C" void libdeflate_b200_ctx_destroy(struct libdeflate_b200_ctx *ctx)
 	cudaFree(ctx->d_stage_out.p);
 	cudaFree(ctx->d_pack.p);
 	cudaFree(ctx->large.p);
+	for (ldb_buf *b : {&ctx->li_scan, &ctx->li_arr, &ctx->li_tok2, &ctx->li_planes, &ctx->li_win, &ctx->li_carry, &ctx->li_hilit, &ctx->li_sums})
+		cudaFree(b->p);
 	cudaFree(ctx->d_params.p);
 	if (ctx->h_pinned.p) cudaFreeHost(ctx->h_pinned.p);
 	if (ctx->h_pinned_tab.p) cudaFreeHost(ctx->h_pinned_tab.p);
@@ -1197,6 +1205,452 @@ extern "C" int libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *c
 	if (r) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(out, ctx->d_stage_out.p, r, cudaMemcpyDeviceToHost, ctx->stream));
 	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
 	*out_nbytes = r;
+	return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// one large stream -> its bytes (large_inflate.cu, inflate_kernel.cu segment mode; DESIGN.md 4.6)
+// ---------------------------------------------------------------------------------
+// Minimum distance in input bytes between two split points (LIBDEFLATE_B200_LARGE_SPLIT_MIN overrides;
+// default 16 KiB, below half of what a compress_large piece compresses to), and the most segments one
+// wave decodes (LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS; the token budget bounds a wave as well).
+static size_t ldb_env_size(const char *name, size_t dflt)
+{
+	if (const char *e = getenv(name)) {
+		long long v = atoll(e);
+		if (v > 0) return (size_t)v;
+	}
+	return dflt;
+}
+
+// host-side bump layout of one device buffer
+struct dev_layout {
+	std::vector<u8> h;
+	size_t take(size_t bytes)
+	{
+		size_t o = h.size();
+		h.resize(o + align_up(bytes ? bytes : 1, 256));
+		return o;
+	}
+	template <typename T> T *at(size_t off) { return (T *)(h.data() + off); }
+};
+
+// segment k of the split list: k = 0 starts at the stream start (wrapper parsed there), k >= 1 at split[k - 1]
+struct li_seg_desc {
+	u64 start;
+	u32 pfx;
+	u32 split_i;
+	size_t room;
+	u64 slot;
+};
+
+// Decodes 'segs' in segment mode.  Arrays go to 'arr' (a region of ctx->li_arr laid out by the caller),
+// tokens to 'tok'.  info (device) receives one ldb_seg_info per segment.
+static int li_decode(libdeflate_b200_ctx *ctx, int format, const ldb_seg_args &g0, const std::vector<li_seg_desc> &segs,
+		     u8 *d_arr, u8 *tok, ldb_inflate_args *a_out, ldb_seg_info **d_info_out)
+{
+	const size_t w = segs.size();
+	dev_layout L;
+	const size_t o_start = L.take(w * 8), o_pfx = L.take(w * 4), o_si = L.take(w * 4), o_room = L.take(w * sizeof(size_t));
+	const size_t o_off = L.take((w + 1) * 8), o_info = L.take(w * sizeof(ldb_seg_info));
+	u64 acc = 0;
+	for (size_t i = 0; i < w; i++) {
+		L.at<u64>(o_start)[i] = segs[i].start;
+		L.at<u32>(o_pfx)[i] = segs[i].pfx;
+		L.at<u32>(o_si)[i] = segs[i].split_i;
+		L.at<size_t>(o_room)[i] = segs[i].room;
+		L.at<u64>(o_off)[i] = acc;
+		acc += segs[i].slot;
+	}
+	L.at<u64>(o_off)[w] = acc;
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_arr, L.h.data(), L.h.size(), cudaMemcpyHostToDevice, ctx->stream));
+	ldb_seg_args g = g0;
+	g.start = (const u64 *)(d_arr + o_start);
+	g.pfx = (const u32 *)(d_arr + o_pfx);
+	g.split_i = (const u32 *)(d_arr + o_si);
+	g.info = (ldb_seg_info *)(d_arr + o_info);
+	ldb_inflate_args a = {};
+	a.out_avail = (const size_t *)(d_arr + o_room);
+	a.overflow_scratch = (u8 *)ctx->inflate_scratch.p;
+	a.tok_base = tok;
+	a.tok_off = (const u64 *)(d_arr + o_off);
+	a.tok_origin = 0;
+	a.first = 0;
+	a.count = w;
+	a.n = w;
+	a.format = format;
+	a.flags = 0;
+	int rc = ldb_reserve_dev(ctx->inflate_scratch, ldb_inflate_scratch_bytes(ctx->cfg, w));
+	if (rc) return rc;
+	a.overflow_scratch = (u8 *)ctx->inflate_scratch.p;
+	rc = ldb_timed_launch(ctx, LDB_K_INFLATE, [&] { return ldb_launch_inflate_seg(a, g, ctx->cfg, ctx->stream); });
+	if (rc) return rc;
+	*a_out = a;
+	*d_info_out = g.info;
+	return 0;
+}
+
+static size_t li_layout_bytes(size_t w) { return w * (8 + 4 + 4 + 8 + 8 + sizeof(ldb_seg_info)) + 8 * 256 + 8; }
+static size_t li_resolve_bytes(size_t w) { return 4 * (w * 8 + 256); }
+
+// Resolves the chunks of a decoded group: lo_dst[i] (NULL: skip) receives the byte / low-plane resolve of chunk
+// i, hi_dst[i] (NULL: skip) the high plane.  lit_pfx: chunks whose literal streams start with the window prefix.
+static int li_resolve(libdeflate_b200_ctx *ctx, const ldb_inflate_args &a0, const std::vector<ldb_seg_info> &info,
+		      const std::vector<u8 *> &lo_dst, const std::vector<u8 *> &hi_dst, const u8 *hilit, u8 *d_arr)
+{
+	const size_t w = info.size();
+	dev_layout L;
+	const size_t o_plo = L.take(w * 8), o_phi = L.take(w * 8), o_clo = L.take(w * 8), o_chi = L.take(w * 8);
+	size_t nhi = 0;
+	for (size_t i = 0; i < w; i++) {
+		L.at<u8 *>(o_plo)[i] = lo_dst[i];
+		L.at<u8 *>(o_phi)[i] = hi_dst[i];
+		L.at<u32>(o_clo)[2 * i] = lo_dst[i] ? info[i].n_rec : 0;
+		L.at<u32>(o_clo)[2 * i + 1] = 0;
+		L.at<u32>(o_chi)[2 * i] = hi_dst[i] ? info[i].n_rec : 0;
+		L.at<u32>(o_chi)[2 * i + 1] = 0;
+		nhi += hi_dst[i] != nullptr;
+	}
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_arr, L.h.data(), L.h.size(), cudaMemcpyHostToDevice, ctx->stream));
+	ldb_inflate_args a = a0;
+	u32 *counter = ldb_inflate_resolve_counter(a, ctx->cfg);
+	a.out_ptrs = (void *const *)(d_arr + o_plo);
+	a.tok_counts = (u32 *)(d_arr + o_clo);
+	LDB_CUDA_CHECK_RET(cudaMemsetAsync(counter, 0, sizeof(u32), ctx->stream));
+	int rc = ldb_timed_launch(ctx, LDB_K_RESOLVE, [&] { return ldb_launch_inflate_resolve(a, ctx->cfg, ctx->stream); });
+	if (rc || !nhi) return rc;
+	a.out_ptrs = (void *const *)(d_arr + o_phi);
+	a.tok_counts = (u32 *)(d_arr + o_chi);
+	LDB_CUDA_CHECK_RET(cudaMemsetAsync(counter, 0, sizeof(u32), ctx->stream));
+	return ldb_timed_launch(ctx, LDB_K_RESOLVE, [&] { return ldb_launch_inflate_resolve_lit(a, hilit, ctx->cfg, ctx->stream); });
+}
+
+extern "C" size_t libdeflate_b200_decompress_large_segments(struct libdeflate_b200_ctx *ctx) { return ctx->li_segments; }
+
+extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
+						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+{
+	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	ctx->li_segments = 0;
+	const u8 *in = (const u8 *)d_in;
+	u8 *out = (u8 *)d_out;
+	const size_t n = in_nbytes;
+	const u32 footer = format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0);
+	const u64 data_end = n >= footer ? n - footer : 0;	// the DEFLATE data ends before the trailer
+	int rc;
+
+	// ---- 1. sync points: every 00 00 FF FF, then split points at least split_min apart ----------------
+	std::vector<u64> split;
+	{
+		const size_t tiles = ldb_sync_scan_tiles(n);
+		if (tiles) {
+			rc = ldb_reserve_dev(ctx->li_scan, tiles * 12 + 512);
+			if (rc) return rc;
+			u32 *d_counts = (u32 *)ctx->li_scan.p;
+			rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_sync_scan_count(in, n, d_counts, tiles, ctx->stream); });
+			if (rc) return rc;
+			std::vector<u32> counts(tiles);
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(counts.data(), d_counts, tiles * 4, cudaMemcpyDeviceToHost, ctx->stream));
+			LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+			std::vector<u64> toff(tiles);
+			u64 total = 0;
+			for (size_t t = 0; t < tiles; t++) { toff[t] = total; total += counts[t]; }
+			if (total) {
+				const size_t o_off = align_up(tiles * 4, 256);
+				const size_t o_cand = o_off + align_up(tiles * 8, 256);
+				rc = ldb_reserve_dev(ctx->li_scan, o_cand + total * 8);
+				if (rc) return rc;
+				u8 *b = (u8 *)ctx->li_scan.p;
+				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(b + o_off, toff.data(), tiles * 8, cudaMemcpyHostToDevice, ctx->stream));
+				rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_sync_scan_write(in, n, (const u64 *)(b + o_off), (u64 *)(b + o_cand), tiles, ctx->stream); });
+				if (rc) return rc;
+				std::vector<u64> cand(total);
+				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(cand.data(), b + o_cand, total * 8, cudaMemcpyDeviceToHost, ctx->stream));
+				LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+				const u64 dmin = ldb_env_size("LIBDEFLATE_B200_LARGE_SPLIT_MIN", 16384);
+				u64 last = 0;
+				for (u64 c : cand)
+					if (c < data_end && c - last >= dmin) { split.push_back(c); last = c; }
+			}
+		}
+	}
+	const size_t nseg = split.size() + 1;
+	// the split list lives at the start of li_scan for the whole call
+	if (!split.empty()) {
+		rc = ldb_reserve_dev(ctx->li_scan, split.size() * 8 + 256);
+		if (rc) return rc;
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_scan.p, split.data(), split.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+	}
+	ldb_seg_args g0 = {};
+	g0.base = in;
+	g0.in_nbytes = n;
+	g0.split = (const u64 *)ctx->li_scan.p;
+	g0.nsplit = (u32)split.size();
+	auto seg_start = [&](size_t k) -> u64 { return k ? split[k - 1] : 0; };
+	auto seg_desc = [&](size_t k, u32 pfx, size_t room) {
+		li_seg_desc d;
+		d.start = seg_start(k);
+		d.pfx = pfx;
+		d.split_i = (u32)(k ? k : 0);
+		d.room = room;
+		const u64 hint_end = k + 1 < nseg ? split[k] : n;
+		d.slot = align_up(pfx + ldb_inflate_tok_cap(hint_end - d.start, out_avail) + 64, 16);
+		return d;
+	};
+
+	// ---- 2..6. waves of consecutive segments, from the current chain segment on ---------------------
+	struct chain_rec { u64 G, len; };
+	std::vector<chain_rec> chain;
+	ldb_large_verdict v = {};
+	v.result = -1;
+	const u64 budget = ldb_token_budget();
+	const size_t wave_max = ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS", (size_t)1 << 20);
+	u64 G = 0;
+	size_t cur = 0;		// the next chain segment
+	rc = ldb_reserve_dev(ctx->li_carry, LDB_SEG_PREFIX);
+	if (rc) return rc;
+	LDB_CUDA_CHECK_RET(cudaMemsetAsync(ctx->li_carry.p, 0, LDB_SEG_PREFIX, ctx->stream));
+	// the one segment whose verdict is the stream's, decoded again with its exact room and prefix
+	auto verdict_of = [&](size_t k) -> int {
+		const u32 pfx = (u32)(G < LDB_SEG_PREFIX ? G : LDB_SEG_PREFIX);
+		li_seg_desc d = seg_desc(k, pfx, out_avail - G);
+		d.slot = 0;		// only the verdict is wanted: every token is counted, none written
+		std::vector<li_seg_desc> one(1, d);
+		int rc2 = ldb_reserve_dev(ctx->li_arr, li_layout_bytes(1));
+		if (rc2) return rc2;
+		ldb_inflate_args a;
+		ldb_seg_info *d_info;
+		rc2 = li_decode(ctx, format, g0, one, (u8 *)ctx->li_arr.p, (u8 *)ctx->li_arr.p, &a, &d_info);
+		if (rc2) return rc2;
+		ldb_seg_info r;
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(&r, d_info, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+		if (r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED)
+			return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment decoded alone disagrees with its chain", __FILE__, __LINE__);
+		v.result = (s32)r.verdict;
+		return 0;
+	};
+	while (v.result < 0) {
+		const size_t k0 = cur;
+		std::vector<li_seg_desc> segs;
+		u64 tok_bytes = 0;
+		for (size_t k = k0; k < nseg && segs.size() < wave_max; k++) {
+			li_seg_desc d = seg_desc(k, k ? LDB_SEG_PREFIX : 0, out_avail);
+			if (!segs.empty() && tok_bytes + d.slot > budget) break;
+			segs.push_back(d);
+			tok_bytes += d.slot;
+		}
+		const size_t w = segs.size(), k1 = k0 + w;
+		// li_arr: decode arrays of the wave | of the re-decode | resolve arrays x 2 | prefix lists x 2 | chain list
+		const size_t lay = li_layout_bytes(w), rlay = li_resolve_bytes(w), plist = w * 8 + 256;
+		const size_t o_dec2 = lay, o_res = 2 * lay, o_pre = o_res + 2 * rlay, o_cs = o_pre + 2 * plist;
+		rc = ldb_reserve_dev(ctx->token_scratch, tok_bytes + 256);
+		if (!rc) rc = ldb_reserve_dev(ctx->li_arr, o_cs + w * sizeof(ldb_chain_seg) + 256);
+		if (rc) return rc;
+		u8 *arr = (u8 *)ctx->li_arr.p;
+		ldb_inflate_args a;
+		ldb_seg_info *d_info;
+		rc = li_decode(ctx, format, g0, segs, arr, (u8 *)ctx->token_scratch.p, &a, &d_info);
+		if (rc) return rc;
+		std::vector<ldb_seg_info> info(w);
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(info.data(), d_info, w * sizeof(ldb_seg_info), cudaMemcpyDeviceToHost, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+
+		// ---- chain plan: follow the stops from the current segment ----
+		std::vector<size_t> wchain;	// wave-local indices of this wave's chain segments
+		std::vector<u64> wG(w);		// their output offsets G_k
+		size_t j = 0;
+		for (;;) {
+			const ldb_seg_info &r = info[j];
+			const size_t k = k0 + j;
+			const bool ok = r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED;
+			if (!ok || r.reach > G || r.out_len > out_avail - G) {
+				// the segment's own limits: its input and output positions are 32-bit
+				if (data_end - seg_start(k) > 0xfffffff0u && r.verdict != LDB_SEG_STOPPED)
+					return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment has more than 4 GiB - 16 of input", __FILE__, __LINE__);
+				if (r.verdict == LDB_INSUFFICIENT_SPACE && out_avail > 0xfffffff0u - segs[j].pfx)
+					return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment has more than 4 GiB - 32 KiB of output", __FILE__, __LINE__);
+				rc = verdict_of(k);
+				if (rc) return rc;
+				break;
+			}
+			wchain.push_back(j);
+			wG[j] = G;
+			chain.push_back({G, r.out_len});
+			G += r.out_len;
+			if (r.verdict == LDB_SUCCESS) {		// the final block: the stream ends here
+				v.actual_in = r.end + footer;
+				v.actual_out = G;
+				v.trailer = r.trailer;
+				v.isize = r.isize;
+				v.result = (flags & 1u) && G != out_avail ? LDB_SHORT_OUTPUT : LDB_SUCCESS;
+				break;
+			}
+			const size_t next = (size_t)r.split_j + 1;
+			if (next >= k1) { cur = next; break; }
+			j = next - k0;
+		}
+		if (v.result > 0) break;	// failed (or SHORT_OUTPUT): the output is not contractual
+
+		// ---- re-decode the chain segments whose tokens overflowed their slots, with exact slots ----
+		std::vector<size_t> redo;
+		for (size_t c : wchain)
+			if (info[c].overflow) redo.push_back(c);
+		ldb_inflate_args a2 = {};
+		std::vector<li_seg_desc> rs;
+		if (!redo.empty()) {
+			u64 bytes = 0;
+			for (size_t c : redo) {
+				li_seg_desc d = segs[c];
+				d.slot = align_up((u64)info[c].n_lit + 4ull * info[c].n_rec + 64, 16);
+				bytes += d.slot;
+				rs.push_back(d);
+			}
+			rc = ldb_reserve_dev(ctx->li_tok2, bytes + 256);
+			if (rc) return rc;
+			ldb_seg_info *d_info2;
+			rc = li_decode(ctx, format, g0, rs, arr + o_dec2, (u8 *)ctx->li_tok2.p, &a2, &d_info2);
+			if (rc) return rc;
+		}
+
+		// ---- symbol planes of the chain segments: lo | hi, each with the 32 KiB prefix in front ----
+		// (segment 0 is decoded with no prefix and resolved straight into out)
+		std::vector<u64> poff(w, 0), plen(w, 0);
+		u64 plane_bytes = 0;
+		u32 max_lit = 0;
+		for (size_t c : wchain) {
+			if (k0 + c == 0) continue;
+			plen[c] = align_up(LDB_SEG_PREFIX + (u64)info[c].out_len + 16, 16);
+			poff[c] = plane_bytes;
+			plane_bytes += (info[c].reach ? 2 : 1) * plen[c];
+			if (info[c].reach && info[c].n_lit > max_lit) max_lit = info[c].n_lit;
+		}
+		rc = ldb_reserve_dev(ctx->li_planes, plane_bytes + 256);
+		if (rc) return rc;
+		u8 *planes = (u8 *)ctx->li_planes.p;
+		if (max_lit) {	// literal stream of the high planes: 1 + j / 256 for the prefix, 0 after it
+			rc = ldb_reserve_dev(ctx->li_hilit, (size_t)max_lit + 64);
+			if (rc) return rc;
+			std::vector<u8> pat(LDB_SEG_PREFIX);
+			for (u32 i = 0; i < LDB_SEG_PREFIX; i++) pat[i] = (u8)(1 + (i >> 8));
+			LDB_CUDA_CHECK_RET(cudaMemsetAsync(ctx->li_hilit.p, 0, (size_t)max_lit + 64, ctx->stream));
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync((u8 *)ctx->li_hilit.p + 16, pat.data(), LDB_SEG_PREFIX, cudaMemcpyHostToDevice, ctx->stream));
+		}
+		const u8 *hilit = max_lit ? (const u8 *)ctx->li_hilit.p + 16 : nullptr;
+		auto lo_of = [&](size_t c) { return k0 + c ? planes + poff[c] : out + wG[c]; };
+		auto hi_of = [&](size_t c) { return k0 + c && info[c].reach ? planes + poff[c] + plen[c] : nullptr; };
+
+		// ---- resolve: group 0 = the wave's decode (minus the overflowed), group 1 = the re-decode ----
+		for (int grp = 0; grp < 2; grp++) {
+			const std::vector<li_seg_desc> &gs = grp ? rs : segs;
+			if (gs.empty()) continue;
+			const size_t gw = gs.size();
+			std::vector<ldb_seg_info> ginfo(gw);
+			std::vector<u8 *> lo(gw, nullptr), hi(gw, nullptr), pre;
+			u8 *tok = grp ? (u8 *)ctx->li_tok2.p : (u8 *)ctx->token_scratch.p;
+			u64 off = 0;
+			for (size_t i = 0; i < gw; i++) {
+				const size_t c = grp ? redo[i] : i;
+				ginfo[i] = info[c];
+				const bool on = k0 + c < k1 && (grp || (!info[c].overflow && std::find(wchain.begin(), wchain.end(), c) != wchain.end()));
+				if (on) {
+					lo[i] = lo_of(c);
+					hi[i] = hi_of(c);
+					if (k0 + c) pre.push_back(tok + off);	// the slot's literal stream starts with the prefix
+				}
+				off += gs[i].slot;
+			}
+			if (!pre.empty()) {
+				u8 *d_pre = arr + o_pre + grp * plist;
+				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_pre, pre.data(), pre.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+				rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_seg_prefix_fill((u8 *const *)d_pre, pre.size(), ctx->stream); });
+				if (rc) return rc;
+			}
+			rc = li_resolve(ctx, grp ? a2 : a, ginfo, lo, hi, hilit, arr + o_res + grp * rlay);
+			if (rc) return rc;
+		}
+
+		// ---- windows through the chain, then symbols -> bytes at out + G_k ----
+		const size_t nc = wchain.size();
+		std::vector<ldb_chain_seg> cs(nc);
+		for (size_t m = 0; m < nc; m++) {
+			const size_t c = wchain[m];
+			const bool rel = k0 + c != 0;
+			cs[m].lo = rel ? lo_of(c) + LDB_SEG_PREFIX : out;
+			const u8 *h = hi_of(c);
+			cs[m].hi = h ? h + LDB_SEG_PREFIX : nullptr;
+			cs[m].dst = rel ? out + wG[c] : nullptr;
+			cs[m].len = info[c].out_len;
+		}
+		rc = ldb_reserve_dev(ctx->li_win, (nc + 1) * (size_t)LDB_SEG_PREFIX);
+		if (rc) return rc;
+		u8 *win = (u8 *)ctx->li_win.p;
+		u8 *d_cs = arr + o_cs;
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_cs, cs.data(), nc * sizeof(ldb_chain_seg), cudaMemcpyHostToDevice, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(win, ctx->li_carry.p, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
+		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_window_chain((const ldb_chain_seg *)d_cs, nc, win, ctx->stream); });
+		if (!rc) rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_substitute((const ldb_chain_seg *)d_cs, nc, win, ctx->stream); });
+		if (rc) return rc;
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_carry.p, win + nc * (size_t)LDB_SEG_PREFIX, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
+		// (the next wave reuses these buffers)
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	}
+	ctx->li_segments = chain.size() ? chain.size() : 1;
+
+	// ---- 7. checksum of the output, in order, against the trailer; the results ----------------------
+	const size_t nch = v.result == LDB_SUCCESS && format != LDB_FMT_RAW ? chain.size() : 0;
+	rc = ldb_reserve_dev(ctx->li_sums, nch * 20 + 1024);
+	if (rc) return rc;
+	u8 *sb = (u8 *)ctx->li_sums.p;
+	const void **d_ptrs = (const void **)sb;
+	size_t *d_lens = (size_t *)(sb + align_up(nch * 8, 256));
+	u32 *d_sums = (u32 *)(sb + 2 * align_up(nch * 8, 256));
+	if (nch) {
+		std::vector<const void *> hp(nch);
+		std::vector<size_t> hl(nch);
+		for (size_t i = 0; i < nch; i++) { hp[i] = out + chain[i].G; hl[i] = chain[i].len; }
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)d_ptrs, hp.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_lens, hl.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
+		if (format == LDB_FMT_GZIP)
+			rc = ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, d_ptrs, d_lens, nullptr, d_sums, nch, ctx->cfg, ctx->stream); });
+		else
+			rc = ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32(d_ptrs, d_lens, nullptr, d_sums, nch, ctx->cfg, ctx->stream); });
+		if (rc) return rc;
+	}
+	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_inflate_finish(d_sums, d_lens, nch, format, v, d_actual_in, d_actual_out, d_result, ctx->stream); });
+}
+
+extern "C" int libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+						      const void *in, size_t in_nbytes, void *out, size_t out_avail,
+						      size_t *actual_in, size_t *actual_out, int32_t *result)
+{
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	stream_quiesce quiesce(ctx);
+	int rc = ldb_reserve_dev(ctx->d_stage_in, in_nbytes + 64);
+	if (!rc) rc = ldb_reserve_dev(ctx->d_stage_out, out_avail + 64);
+	if (!rc) rc = ldb_reserve_dev(ctx->d_params, 256);
+	if (rc) return rc;
+	// (both sides keep their 16-byte alignment phase on the device)
+	u8 *d_in = (u8 *)ctx->d_stage_in.p + ((uintptr_t)in & 15);
+	u8 *d_out = (u8 *)ctx->d_stage_out.p + ((uintptr_t)out & 15);
+	size_t *d_res = (size_t *)ctx->d_params.p;	// actual_in, actual_out, result
+	if (in_nbytes) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_in, in, in_nbytes, cudaMemcpyHostToDevice, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaMemsetAsync(d_res, 0, 3 * sizeof(size_t), ctx->stream));
+	rc = libdeflate_b200_decompress_large(ctx, format, flags, d_in, in_nbytes, d_out, out_avail, d_res, d_res + 1, (int32_t *)(d_res + 2));
+	if (rc) return rc;
+	size_t h[3];
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(h, d_res, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	const int32_t r = (int32_t)h[2];
+	if (r == LDB_SUCCESS && h[1]) {
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(out, d_out, h[1], cudaMemcpyDeviceToHost, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	}
+	if (result) *result = r;
+	if (actual_in) *actual_in = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[0] : 0;
+	if (actual_out) *actual_out = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[1] : 0;
 	return 0;
 }
 

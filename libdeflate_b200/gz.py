@@ -75,6 +75,27 @@ def decompress_members(api, data):
     return b"".join(out)
 
 
+def decompress_members_large(ctx, data):
+    """Any multi-member gzip file, each member through decompress_large: a member with sync points (zlib /
+    pigz flushes, compress_large) is decoded by the whole GPU, one without them on one lane.  Same output
+    loop as decompress_members()."""
+    out, pos = [], 0
+    while pos < len(data):
+        avail = max(4 * (len(data) - pos), 1 << 16)
+        while True:
+            res, piece, ain, _aout = ctx.decompress_large(data[pos:], avail, ldb.GZIP)
+            if res != 3:        # LIBDEFLATE_INSUFFICIENT_SPACE
+                break
+            if avail > 1032 * (len(data) - pos) + (1 << 16):
+                break           # more room cannot help: DEFLATE expands at most ~1032:1
+            avail *= 2
+        if res != 0:
+            raise ValueError("decompression failed: libdeflate_result %d at byte %d" % (res, pos))
+        out.append(piece)
+        pos += ain
+    return b"".join(out)
+
+
 def main(argv=None, ctx=None, api=None):
     ap = argparse.ArgumentParser(prog="python -m libdeflate_b200.gz", description=__doc__.split("\n\n")[1])
     ap.add_argument("-d", "--decompress", action="store_true")
@@ -92,7 +113,7 @@ def main(argv=None, ctx=None, api=None):
             try:
                 out = decompress_bytes(ctx, data)
             except ValueError:
-                out = decompress_members(api or ldb.Api(), data)     # not blocked: member by member
+                out = decompress_members_large(ctx, data)     # not blocked: member by member
             dst = path[:-3] if path.endswith(".gz") else path + ".out"
         else:
             out = compress_bytes(ctx, data, level)
