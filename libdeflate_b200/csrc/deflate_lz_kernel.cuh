@@ -23,10 +23,11 @@
 //       - guided search: every thread walks dynamically assigned runs of 16 or 32
 //         positions like the reference's lazy parser, but every position ends up with a
 //         (length, distance), which is what lets the parse itself be parallel,
-//       - exact parallel lazy parse: per-window pointer jumping gives "where does a
-//         parse entering at lane e leave this 32-position window" for all e at once,
-//         the windows are chained group-parallel, __reduce_or_sync marks the visited
-//         positions, a prefix sum places the tokens,
+//       - exact parallel lazy parse: a step table (1 or the match length per position),
+//         then one thread per 32-position window walks it from a guessed entry lane;
+//         rounds re-walk the windows whose entry the previous window's exit changed
+//         until none does (trajectories merge within a token or two, so few rounds),
+//         a prefix sum places the tokens,
 //   * tokens and per-position results go to a per-CTA buffer in global memory (L2
 //     resident), symbol histograms stay in shared memory,
 //   * per block (32 KiB of input): Huffman codes (length-limited to 15; parallel except
@@ -66,15 +67,20 @@
 // Levels 1-9 run two warp groups: warps [0, LZ_PWARPS) parse pass k and flush its block while the
 // others search pass k + 1, then join that search.  The block flush needs one thread per symbol of
 // the 320-symbol alphabets and of the <= 320 code lengths the precode run-length codes.  Deflate
-// kernel at L6, 65536 x 64 KiB on an H100 80GB HBM3 at a 400 W power limit: 10 / 12 / 14 / 16 warps
-// 293.0 / 288.6 / 287.8 / 294.8 ms (one-group order: 301.3 ms).
+// kernel at L6, 65536 x 64 KiB, with the speculative-walk parse, on an H100 80GB HBM3 at 700 W:
+// 10 / 12 / 14 warps 262.1 / 258.8 / 266.4 ms.
 #ifndef LZ_PWARPS
-#define LZ_PWARPS    14
+#define LZ_PWARPS    12
 #endif
 #define LZ_BAR_P     1				// named barrier of the parse/flush group
 #ifndef LZ_PF
 #define LZ_PF        4				// parse: windows of per-position results in flight per warp
 #endif
+// parse: speculative walk rounds before one thread finishes the pass in order (adversarial inputs)
+#ifndef LZ_SPEC_ROUNDS
+#define LZ_SPEC_ROUNDS 4
+#endif
+static_assert(LZ_SPEC_ROUNDS >= 1 && LZ_SPEC_ROUNDS <= 14, "round statistic buckets");
 static_assert(LZ_PWARPS >= 10 && LZ_PWARPS < LZ_WARPS, "parse/flush group: 320..LZ_THREADS-32 threads");
 
 // shared memory layout
@@ -84,10 +90,9 @@ static_assert(LZ_PWARPS >= 10 && LZ_PWARPS < LZ_WARPS, "parse/flush group: 320..
 #define LZ_SM_R      (LZ_SM_HEAD + 2 * (1 << LZ_HASH_BITS))	// 12 KiB multi-purpose region:
 #define LZ_SM_VIS    (LZ_SM_R)					//   parse: u32[NWIN] visited masks
 #define LZ_SM_TOKOFF (LZ_SM_R + 4096)				//   parse: u32[NWIN + 16] token offsets
-#define LZ_SM_ENTRY  (LZ_SM_R + 8320)				//   parse: u8[NWIN] entry lane per window
+#define LZ_SM_ENTRY  (LZ_SM_R + 8320)				//   parse: u8[2][NWIN] entry lane per window, by round parity
 #define LZ_SM_ESCAN  (LZ_SM_R + 9344)				//   emission: scan scratch u32[80]
-#define LZ_SM_GEXIT  (LZ_SM_R + 9728)				//   parse: u16[WARPS * 32] group exits
-#define LZ_SM_GENTRY (LZ_SM_R + 11776)				//   parse: u32[WARPS] group entries (WARPS <= 32)
+#define LZ_SM_GEXIT  (LZ_SM_R + 9728)				//   parse: u16[2][NWIN] exit per window, by round parity
 #define LZ_SM_ITEMS  (LZ_SM_R + 12288)				// u16[512] precode items
 #define LZ_SM_FREQ   (LZ_SM_ITEMS + 1024)			// u32[288 + 32]
 #define LZ_SM_LENS   (LZ_SM_FREQ + 4 * 320)			// u8[320]
@@ -130,7 +135,10 @@ struct lz_vars {
 	u32 pre_lens_packed[3];
 	u32 tma_phase;
 	u32 dict, nonfinal;	// the chunk's ldb_deflate_args::piece fields
+	u32 spec_last;		// parse: last round in which a window's entry changed
+	u32 spec_first;		// parse: first window the last allowed round changed
 };
+static_assert(sizeof(lz_vars) <= 256, "lz_vars fits its shared-memory slot");
 
 struct lz_params {
 	int depth, nice, lazy;
@@ -342,6 +350,23 @@ __device__ unsigned long long ldb_lz_timing[2][16];
 #define LZ_T(k) do { if (tid == 0 || tid == 32 * LZ_PWARPS) { long long t_ = clock64(); tacc[k] += t_ - tlast; tlast = t_; } } while (0)
 #else
 #define LZ_T(k) do { } while (0)
+#endif
+
+#ifdef LZ_SPEC_STATS
+// tuning builds only: parsed passes by the round r that found no entry to change (r = 1: every guess of
+// round 0 was right), bucket LZ_SPEC_ROUNDS + 1: the pass needed the in-order tail
+__device__ unsigned long long ldb_lz_spec_rounds[16];
+extern "C" __attribute__((visibility("default"))) void ldb_lz_spec_stats(unsigned long long *out, int reset)
+{
+#ifdef LDB_EMU
+	for (int i = 0; i < 16; i++) { out[i] = ldb_lz_spec_rounds[i]; if (reset) ldb_lz_spec_rounds[i] = 0; }
+#else
+	unsigned long long z[16] = {};
+	cudaDeviceSynchronize();
+	cudaMemcpyFromSymbol(out, ldb_lz_spec_rounds, sizeof(z));
+	if (reset) cudaMemcpyToSymbol(ldb_lz_spec_rounds, z, sizeof(z));
+#endif
+}
 #endif
 
 // Lanes holding the same NBITS-bit key, from NBITS ballots (__match_any_sync gives the same mask
@@ -755,7 +780,6 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 	u8 *entryt = sm + LZ_SM_ENTRY;
 	u32 *escan = (u32 *)(sm + LZ_SM_ESCAN);
 	u16 *gexit = (u16 *)(sm + LZ_SM_GEXIT);
-	u32 *gentry = (u32 *)(sm + LZ_SM_GENTRY);
 	u32 *freq = (u32 *)(sm + LZ_SM_FREQ);
 	u8 *lens = sm + LZ_SM_LENS;
 	u16 *codes = (u16 *)(sm + LZ_SM_CODES);
@@ -771,7 +795,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 	u16 *items = (u16 *)(sm + LZ_SM_ITEMS);				// precode items (<= 320 + slack)
 	// per-position results of the current pass live in this CTA's global scratch
 	u8 *gs = a.scratch + 256 + (size_t)blockIdx.x * LZ_GS_BYTES;
-	u32 *res = (u32 *)(gs + LZ_GS_RES);	// per position: match length | (distance-1 | decision flag << 15) << 16
+	u32 *res = (u32 *)(gs + LZ_GS_RES);	// per position: match length | (distance-1 | DP decision flag << 15) << 16
 	u32 *tokbuf = (u32 *)(gs + LZ_GS_TOK);
 	u32 *costg = (u32 *)(gs + LZ_GS_COST);
 	u32 *mlist = (u32 *)(gs + LZ_GS_MLIST);
@@ -882,13 +906,15 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		// ---- exact parallel parse of one pass (positions [pb0, ppend), results at res[aoff + i]).
 		// forced: the DP already decided (flag set on matches); otherwise the lazy rule decides.
 		// exitt: 16 Ki u16 of scratch in shared memory -- dead link slots (see lz_insert_pass_par and the
-		// pass loop below)
+		// pass loop below) -- holds the step table: 1 for a literal, else the match length.  Position k of
+		// window w sits at w * 32 + (k ^ (w & 31)): e1's coalesced stores and the walks of e2, where 32
+		// threads read the same lane of 32 consecutive windows, are free of bank conflicts.
 		auto parse_pass = [&](const u32 pb0, const u32 ppend, const u32 aoff, const bool forced, u16 *exitt) {
-			// (e1) per-window decisions + "exit position for every entry lane" by pointer jumping
+			// (e1) per-position decisions -> step table
 			const u32 nwin = (ppend - pb0 + 31) >> 5;
 			// (the per-position results live in L2: every warp walks its contiguous group of windows
-			// [wbeg, wend) -- the groups of e2 -- with the loads of LZ_PF windows in flight, and the last
-			// lane takes the next window's first two results from those loads by shuffle)
+			// [wbeg, wend) with the loads of LZ_PF windows in flight, and the last lane takes the next
+			// window's first two results from those loads by shuffle)
 			const u32 min_len = v->min_len, far4 = v->far4_dist;
 			const u32 G = (nwin + GW - 1) / GW;			// windows per group
 			const u32 wbeg = warp * G, wend = wbeg + G < nwin ? wbeg + G : nwin;
@@ -913,7 +939,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				// (a shortest-possible match at a long distance costs more bits than its literals: the
 				// reference's rule for length 3 beyond 8 KiB, deflate_compress.c:2666-2668, restated for our
 				// minimum length 4)
-				bool is_match = forced ? ((L0 >= 3) && p < ppend) : (L0 >= min_len && p < ppend && !(L0 == 4 && O0 > far4));
+				bool is_match = forced ? ((W0 >> 31) && p < ppend) : (L0 >= min_len && p < ppend && !(L0 == 4 && O0 > far4));
 				if (!forced && is_match && P.lazy && p + 1 < ppend) {
 					// ref: deflate_compress.c:2722-2725 -- prefer the next position's match if clearly better
 					if (L1 >= L0 && L0 < (u32)P.nice &&
@@ -927,139 +953,130 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 							is_match = false;
 					}
 				}
-				u32 step = is_match ? L0 : 1;
-				// decision flag in the top bit; the neighbour that reads res[aoff + i] for its lazy test
-				// masks it off, and it only reads -- the flag is published after this warp's reads
-				__syncwarp();
-				if (is_match && !forced) res[aoff + i] = L0 | (((O0 - 1) | 0x8000u) << 16);
-				u32 j = lane + step;
-#pragma unroll
-				for (int k = 0; k < 5; k++) {
-					u32 t = __shfl_sync(LDB_FULL_MASK, j, j & 31);
-					if (j < 32) j = t;
-				}
-				if (p < ppend) exitt[i] = (u16)j;
+				// (positions at or past ppend are literals: the walks need no bounds test)
+				exitt[w * 32 + (lane ^ (w & 31))] = (u16)(is_match ? L0 : 1);
 			}
 			gsync();
 			LZ_T(8);
-			// (e2) chain the windows.  A serial walk over all windows costs ~300 cycles per window on
-			// one warp, so it is split: (a) every warp composes the exits of ITS group of windows for
-			// all 32 possible entry lanes of the group's first window (per-lane shuffles), (b) warp 0
-			// chains the groups, (c) every warp re-walks its group along the one real trajectory and
-			// records the entry lane of each window.
-			{
-				const u32 wg0 = wbeg;				// first window of my group
-				const u32 gstart = wg0 * 32;				// pass-relative position
-				// (a) exits of the group for entries gstart + lane
-				{
-					u32 pos = gstart + lane;
-					for (u32 k0 = 0; k0 < G; k0 += 8) {
-						u32 ex[8];
-#pragma unroll
-						for (int k = 0; k < 8; k++) {
-							u32 w = wg0 + k0 + k;
-							u32 i = w * 32 + lane;
-							ex[k] = (k0 + k < G && w < nwin && pb0 + i < ppend) ? exitt[i] : (lane + 1);
-						}
-#pragma unroll
-						for (int k = 0; k < 8; k++) {
-							u32 w = wg0 + k0 + k;
-							u32 x = __shfl_sync(LDB_FULL_MASK, ex[k], pos & 31);
-							if (k0 + k < G && w < nwin && (pos >> 5) == w) pos = (w << 5) + x;
-						}
-					}
-					gexit[warp * 32 + lane] = (u16)(pos > 0xffff ? 0xffff : pos);
+			// (e2) which positions does the one real parse visit?  One thread per window walks the step
+			// table from an entry lane to the first position past the window, keeps the visited set in a
+			// register and publishes it to vis[w], the entry lane to ent[w] (0xff: the parse jumps over the
+			// window) and the exit (pass-relative position) to wx[w].  Round 0 enters every window at lane
+			// 0 (the window of parse_entry at its lane, the ones before it not at all).  Round r re-derives
+			// every entry from round r - 1: the nearest earlier window with an entry (a token is <= 258
+			// long, so it is at most 9 back) exits into this window or past it.  A window whose entry
+			// changed walks again, and stops where it lands on its old visited set: the rest of its walk,
+			// and its exit, are the old ones.  The search gives every position covered by a match that
+			// match at the same distance, so two walks through a window meet within a token or two and
+			// most passes settle in round 1 or 2.  A round that changes nothing is a fixed point, which is
+			// the serial parse by induction from the first window.  Where walks never merge (every
+			// position in a long match of its own) a correction moves one window per round, so after
+			// LZ_SPEC_ROUNDS rounds one thread follows the parse from the first window that round changed
+			// to the end of the pass: one shared load per token and a store per window.  ent and wx alternate between two buffers
+			// by round parity; vis[w] is only touched by window w's thread until the end.
+			const u32 pe = v->parse_entry - pb0, we = pe >> 5;	// parse entry, pass-relative, and its window
+			auto walk = [&](u32 w, u32 k, u32 stop, u32 &m) -> u32 {	// -> landing lane (>= 32: past the window)
+				const u16 *st = exitt + w * 32;
+				const u32 sw = w & 31;
+				m = 0;
+				while (k < 32 && !((stop >> k) & 1)) {
+					m |= 1u << k;
+					k += st[k ^ sw];
 				}
-				gsync();
-				// (b) chain the groups (warp 0, all lanes redundantly; lane 0 publishes)
-				if (warp == 0) {
-					u32 e = v->parse_entry - pb0;	// pass-relative
-					for (u32 g = 0; g < GW; g++) {
-						const u32 gs = g * G * 32, ge = (g + 1) * G * 32;
-						u32 ent = 0xffffffffu;
-						if (e < ge && gs < (nwin << 5) && pb0 + e < ppend) {
-							ent = e;
-							if (e < gs + 32) {
-								e = gexit[g * 32 + (e - gs)];
-							} else {
-								// entered past the group's first window (a long match jumped in): walk it
-								for (u32 w = e >> 5; w < (g + 1) * G && w < nwin; w++) {
-									if ((e >> 5) == w) {
-										u32 i = w * 32 + (e & 31);
-										u32 x = pb0 + i < ppend ? exitt[i] : ((e & 31) + 1);
-										e = (w << 5) + x;
-									}
-								}
-							}
-						}
-						if (lane == 0) gentry[g] = ent;
-					}
-					u32 fin = pb0 + e;
-					if (fin < ppend) fin = ppend;
-					__syncwarp();	// every lane has read parse_entry (racecheck: read/write by different lanes)
-					if (lane == 0) v->parse_entry = fin;
+				return k;
+			};
+			// window w (entry oe, exit ox) now enters at ne: new visited set to vis[w], returns its exit
+			auto rewalk = [&](u32 w, u32 oe, u32 ne, u32 ox) -> u32 {
+				u32 m = 0;
+				if (ne != 0xff) {
+					const u32 old = oe != 0xff ? vis[w] : 0;
+					const u32 k = walk(w, ne, old, m);
+					if (k < 32) m |= old & ~((1u << k) - 1);
+					else ox = w * 32 + k;
 				}
+				vis[w] = m;
+				return ox;
+			};
+			// entry of window w from the state (e, x); 0xfe: undecided by it, keep the window's own
+			auto derive = [&](u32 w, const u8 *e, const u16 *x) -> u32 {
+				if (w <= we) return w < we ? 0xff : (pe & 31);
+				for (u32 d = 1; d <= 9 && d <= w - we; d++) {
+					if (e[w - d] == 0xff) continue;
+					const u32 xw = x[w - d] >> 5;
+					return xw == w ? (x[w - d] & 31) : (xw > w ? 0xff : 0xfe);
+				}
+				return 0xfe;
+			};
+			u8 *ent = entryt;
+			u16 *wx = gexit;
+			for (u32 w = tid; w < nwin; w += GT) {
+				const u32 e0 = w < we ? 0xff : (w == we ? (pe & 31) : 0);
+				ent[w] = (u8)e0;
+				wx[w] = (u16)rewalk(w, 0xff, e0, 0);
+			}
+			if (tid == 0) { v->spec_last = 0; v->spec_first = 0xffffu; }
+			gsync();
+			u32 r = 1;
+			for (;; r++) {
+				const u8 *pent = ent;
+				const u16 *pwx = wx;
+				ent = entryt + (r & 1) * LZ_NWIN;
+				wx = gexit + (r & 1) * LZ_NWIN;
+				bool changed = false;
+				for (u32 w = tid; w < nwin; w += GT) {
+					const u32 oe = pent[w], ox = pwx[w];
+					u32 ne = derive(w, pent, pwx);
+					if (ne == 0xfe) ne = oe;
+					u32 nx = ox;
+					if (ne != oe) {
+						nx = rewalk(w, oe, ne, ox);
+						changed = true;
+						if (r == LZ_SPEC_ROUNDS) atomicMin(&v->spec_first, w);
+					}
+					ent[w] = (u8)ne;
+					wx[w] = (u16)nx;
+				}
+				if (changed) v->spec_last = r;
 				gsync();
-				// (c) entry lane of every window of my group along the real trajectory
-				{
-					u32 pos = gentry[warp];
-					for (u32 k0 = 0; k0 < G; k0 += 8) {
-						u32 ex[8];
-#pragma unroll
-						for (int k = 0; k < 8; k++) {
-							u32 w = wg0 + k0 + k;
-							u32 i = w * 32 + lane;
-							ex[k] = (k0 + k < G && w < nwin && pb0 + i < ppend) ? exitt[i] : (lane + 1);
-						}
-#pragma unroll
-						for (int k = 0; k < 8; k++) {
-							u32 w = wg0 + k0 + k;
-							if (k0 + k < G && w < nwin) {
-								bool inside = pos != 0xffffffffu && (pos >> 5) == w && pb0 + pos < ppend;
-								u32 x = __shfl_sync(LDB_FULL_MASK, ex[k], pos & 31);
-								if (lane == 0) entryt[w] = inside ? (u8)(pos & 31) : 0xff;
-								if (inside) pos = (w << 5) + x;
+				if (v->spec_last < r) break;	// (a thread already in round r + 1 may have raised it)
+				if (r == LZ_SPEC_ROUNDS) {
+					// windows up to the first one this round changed are settled: follow the parse
+					// from the last of them that it enters, one token at a time
+					if (tid == 0) {
+						u32 w = v->spec_first, pos = 0;
+						while (w > we && ent[w] == 0xff) w--;
+						pos = wx[w];
+						for (w++; w < nwin; w++) {
+							u32 e = 0xff, m = 0;
+							if ((pos >> 5) == w) {
+								e = pos & 31;
+								pos = w * 32 + walk(w, e, 0, m);
+								wx[w] = (u16)pos;
 							}
+							ent[w] = (u8)e;
+							vis[w] = m;
 						}
 					}
+					r++;
+					break;
 				}
 			}
-			gsync();
 			LZ_T(9);
-			// (e3) visited sets per window (loads in flight as in e1)
-			auto e3_load = [&](u32 w) -> u32 {
-				const u32 i = w * 32 + lane;
-				return w < nwin && entryt[w] != 0xff && pb0 + i < ppend ? res[aoff + i] : 0;
-			};
-#pragma unroll
-			for (int k = 0; k < LZ_PF; k++) q[k] = e3_load(wbeg + k);
-			for (u32 w = wbeg; w < wend; w++) {
-				const u32 e = entryt[w], rw = q[0];
-#pragma unroll
-				for (int k = 0; k + 1 < LZ_PF; k++) q[k] = q[k + 1];
-				q[LZ_PF - 1] = e3_load(w + LZ_PF);
-				u32 V = 0;
-				if (e != 0xff) {
-					u32 step = (rw & 0x80000000u) ? (rw & 0xffff) : 1;
-					u32 j = lane + step;
-					u32 jk[5];
-#pragma unroll
-					for (int k = 0; k < 5; k++) {
-						jk[k] = j;
-						u32 t = __shfl_sync(LDB_FULL_MASK, j, j & 31);
-						if (j < 32) j = t;
-					}
-					V = 1u << e;
-#pragma unroll
-					for (int k = 4; k >= 0; k--) {
-						u32 contrib = (((V >> lane) & 1) && jk[k] < 32) ? (1u << jk[k]) : 0;
-						V |= __reduce_or_sync(LDB_FULL_MASK, contrib);
-					}
-					// positions at or beyond the end of the pass are not tokens of this block
-					const u32 wbase = pb0 + w * 32;
-					if (wbase + 32 > ppend) V &= ppend > wbase ? ((1u << (ppend - wbase)) - 1) : 0;
+			if (tid == 0) {
+#ifdef LZ_SPEC_STATS
+				atomicAdd(&ldb_lz_spec_rounds[r], 1ull);
+#endif
+				// the next pass starts where the last window the parse enters is left
+				u32 fin = pe;
+				for (u32 w = nwin; w > we;) {
+					w--;
+					if (ent[w] != 0xff) { fin = wx[w]; break; }
 				}
-				if (lane == 0) vis[w] = V;
+				fin += pb0;
+				v->parse_entry = fin < ppend ? ppend : fin;
+				// positions at or beyond the end of the pass are not tokens of this block
+				const u32 part = (ppend - pb0) & 31;
+				if (part) vis[nwin - 1] &= (1u << part) - 1;
 			}
 			gsync();
 			LZ_T(10);
@@ -1100,7 +1117,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					u32 idx = tbase + tokoff[w] + __popc(V & ((1u << lane) - 1));
 					u32 off = (ro & 0x7fff) + 1;
 					// (a match that does not fit the data would be a bug upstream; never emit one)
-					if ((ro & 0x8000) && len >= 3 && len <= 258 && off <= pb0 + i && pb0 + i + len <= n) {
+					if (exitt[w * 32 + (lane ^ (w & 31))] > 1 && len >= 3 && len <= 258 && off <= pb0 + i && pb0 + i + len <= n) {
 						tokbuf[idx] = 0x80000000u | ((len - 3) << 15) | (off - 1);
 						atomicAdd(&freq[257 + lz_len_slot(len)], 1u);
 						atomicAdd(&freq[288 + lz_off_slot(off)], 1u);
@@ -1812,7 +1829,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 
 		// Pipe: step s loads and inserts pass s (whole CTA); then warps [0, GT) parse pass s - 1 and flush
 		// its block, the others search pass s, and the first group joins that search when it is done.
-		// res[] holds the two passes in flight by parity; the parse's exit table for pass k lives in the
+		// res[] holds the two passes in flight by parity; the parse's step table for pass k lives in the
 		// link slots of pass k + 2: insert(k + 1) used them as list scratch and is done with them, and no
 		// chain of pass k + 1 reaches that far back (they belong to positions >= 48 Ki back).
 		// (the passes of the dictionary, step < LZ_DICT / LZ_PASS, are only loaded and inserted)
@@ -1960,7 +1977,7 @@ extern "C" __attribute__((visibility("default"))) void ldb_lz_timing_dump(void)
 	cudaMemcpyFromSymbol(h, ldb_lz_timing, sizeof(h));
 	cudaMemcpyToSymbol(ldb_lz_timing, z, sizeof(z));
 	const char *names[16] = {"loads+first", "search", "parse e5", "insert: linking", "huffman", "precode", "cost+emit", "chunk pro/epilogue",
-				 "parse e1", "parse e2", "parse e3", "parse e4", "insert: hashing", "insert: slice lists", "wait at join", ""};
+				 "parse e1 steps", "parse e2 walks", "parse e3 exit", "parse e4", "insert: hashing", "insert: slice lists", "wait at join", ""};
 	const char *who[2] = {"thread 0 (parse/flush group; levels 10-12: whole CTA)", "first thread of the search group"};
 	for (int g = 0; g < 2; g++) {
 		unsigned long long tot = 0;

@@ -1,10 +1,10 @@
 """A/B timing of the deflate kernel of two library builds, alternated in one process on one GPU.
 
-    python scripts/ab_deflate.py LIB_A LIB_B [--rounds 3] [--out DIR]
+    python scripts/ab_deflate.py LIB_A LIB_B [--rounds 3] [--data-class 0] [--legs ...] [--out DIR]
 
 Both libraries compress the same device-resident synthetic batches (bench/synth.c class 0, the
-bench corpus); every round times each library once per leg, A then B, so that drift of the card
-shows up in both.  Legs: the bench shape (65 536 x 64 KiB, gzip level 6), levels 1 and 9 on a
+bench corpus, unless --data-class picks another of its six classes); every round times each library
+once per leg, A then B, so that drift of the card shows up in both.  Legs: the bench shape (65 536 x 64 KiB, gzip level 6), levels 1 and 9 on a
 quarter of it, and 528 x 1 MiB at level 12 (four waves of the 132 CTAs).  Reported: deflate kernel
 ms per launch (library event pairs), and whether the two libraries' compressed sizes and a sample of
 their streams agree byte for byte.
@@ -84,6 +84,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--launches", type=int, default=3, help="timed launches per library, leg and round")
     ap.add_argument("--legs", default=",".join(name for name, *_ in LEGS))
+    ap.add_argument("--data-class", type=int, default=0, choices=range(6), help="bench/synth.c class of the inputs")
     ap.add_argument("--out", default=None, help="directory for ab_deflate.json")
     args = ap.parse_args()
     try:
@@ -92,12 +93,12 @@ def main():
     except Exception:
         gpu = "unknown"
     synth = bench.load_synth()
-    report = {"gpu": gpu, "lib_a": args.lib_a, "lib_b": args.lib_b, "legs": {}}
+    report = {"gpu": gpu, "lib_a": args.lib_a, "lib_b": args.lib_b, "data_class": args.data_class, "legs": {}}
     for name, level, n, chunk in LEGS:
         if name not in args.legs.split(","):
             continue
         pin = ctypes.create_string_buffer(n * chunk)
-        synth.synth_fill(pin, chunk, 0, n, 0, os.cpu_count() or 1)
+        synth.synth_fill(pin, chunk, 0, n, args.data_class, os.cpu_count() or 1)
         sides = [Side(args.lib_a, pin, n, chunk), Side(args.lib_b, pin, n, chunk)]
         del pin
         ms = [[], []]
@@ -118,7 +119,8 @@ def main():
     print(json.dumps(report))
     if args.out:
         os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "ab_deflate.json"), "w") as f:
+        name = "ab_deflate.json" if args.data_class == 0 else "ab_deflate_class%d.json" % args.data_class
+        with open(os.path.join(args.out, name), "w") as f:
             json.dump(report, f, indent=1)
 
 
