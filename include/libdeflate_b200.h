@@ -249,8 +249,13 @@ libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *ctx, int format,
  * libdeflate_b200_compress_large, at every flush by zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH, and between pigz's
  * blocks.  Segments that start at such points (at least LIBDEFLATE_B200_LARGE_SPLIT_MIN input bytes apart,
  * default 16384) are decoded at once; a segment is accepted only when the decode from the true stream
- * start reaches its start, so every result is the serial decode's.  A stream without sync points is one
- * segment: one decode lane, as libdeflate_b200_decompress_batch would run it.
+ * start reaches its start, so every result is the serial decode's.  A stream without sync points (gzip,
+ * plain zlib.compress, libdeflate, the classic calls) is split at block boundaries found by a bit-level scan:
+ * non-final dynamic-Huffman headers and the ends of stored blocks, each a guess that the same chain proves
+ * or rejects (a speculative segment gives up LIBDEFLATE_B200_LARGE_OVERRUN bytes, default 4 MiB, past its
+ * next split point).  Such a stream is searched from 4 x LIBDEFLATE_B200_LARGE_SPLIT_MIN bytes of DEFLATE
+ * data on.  Only a stream with neither sync points nor findable block starts (fixed-Huffman blocks only, a
+ * single block) is one segment: one decode lane, as libdeflate_b200_decompress_batch would run it.
  *
  * Result, actual_in and actual_out are exactly those of libdeflate_{deflate,zlib,gzip}_decompress_ex on
  * the whole buffer (gzip: the first member; actual_in tells where a next member starts).  Flags as in

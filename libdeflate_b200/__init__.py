@@ -402,7 +402,8 @@ class Context:
         return ctypes.string_at(out, r.value) if r.value else None
 
     def decompress_large(self, data, out_avail, fmt=RAW, exact=False):
-        """ONE stream decoded by the whole GPU, split at its sync points (result, bytes or None, actual_in,
+        """ONE stream decoded by the whole GPU, split at its sync points or, without them, at the block starts a
+        bit-level scan finds (result, bytes or None, actual_in,
         actual_out) -- the tuple decompress_batch_host gives for the same stream."""
         addr, n, keep = _buf_ptr(data)
         out = ctypes.create_string_buffer(max(out_avail, 1))

@@ -922,11 +922,11 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 // Segment mode (SEG, decompress_large): chunk c is a segment of ONE stream, described by g (ldb_common.cuh).
 // The batch instance (SEG = false) compiles to the code it had before the mode existed.
 
-// a non-final empty stored block has ended at byte 'next' of the segment: is that a split point at or
-// after the segment's next one?  (The index passes split points that lie before the block end.)
-__device__ __forceinline__ bool inf_seg_stop(inf_lane &s, const ldb_seg_args &g, u32 next)
+// a block header starts at bit e of the whole input: is that a split point at or after the segment's next
+// one?  (The index passes split points that lie before the header.)  At sync points only the header after
+// a non-final empty stored block is asked, so that a false sync point never stops a true decode.
+__device__ __forceinline__ bool inf_seg_stop(inf_lane &s, const ldb_seg_args &g, u64 e)
 {
-	const u64 e = s.seg_base + next;
 	while (s.split_i < g.nsplit && g.split[s.split_i] < e) s.split_i++;
 	return s.split_i < g.nsplit && g.split[s.split_i] == e;
 }
@@ -974,7 +974,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 					}
 				}
 			} else if (verdict == LDB_SEG_STOPPED) {
-				r.end = s.seg_base + (P >> 3);
+				r.end = 8 * s.seg_base + P;	// the split point, in bits
 			}
 			if (verdict == LDB_SUCCESS || verdict == LDB_SEG_STOPPED) {
 				const bool fits = inf_seg_fits(s, 8);
@@ -1037,6 +1037,18 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 		// through it once per decode quantum.
 #pragma unroll 1
 		for (int rep = 0; rep < 4; rep++) {
+			// segment mode, once per decode quantum: a speculative segment whose input has passed its next split
+			// point by more than g.overrun bits gives up (real blocks are far shorter; a segment that started at a
+			// false candidate may otherwise decode garbage to the end of the input)
+			if constexpr (SEG) {
+				if (rep == 0 && g.overrun && s.chunk != a.first && s.state != ST_IDLE && s.state != ST_DONE) {
+					const u32 si = g.split_i[s.chunk];
+					if (si < g.nsplit && 8 * s.seg_base + inf_bits_consumed(s) > g.split[si] + g.overrun) {
+						s.verdict = LDB_SEG_ABANDONED;
+						s.state = ST_DONE;
+					}
+				}
+			}
 			// (0) streams that have ended
 			if (s.state == ST_DONE) finish();
 			// (1) idle lanes fetch new chunks
@@ -1070,7 +1082,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 							s.reach = 0;
 							s.split_i = g.split_i[c];
 							u32 footer = a.format == LDB_FMT_GZIP ? 8 : (a.format == LDB_FMT_ZLIB ? 4 : 0);
-							u64 skip = st;
+							u64 skip = st >> 3;
 							if (st == 0) {	// the stream start: the wrapper header is parsed here only
 								const u32 hdr = inf_parse_wrapper(g.base, g.in_nbytes, a.format, &footer);
 								skip = hdr == 0xffffffffu ? ~(u64)0 : hdr;
@@ -1092,6 +1104,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 								s.in_nal = s.in_a0 + s.in_n;
 								s.hdr_bytes = 0;
 								inf_bits_init(s, 0);
+								s.bitpos += (u32)(st & 7);	// a block may start at any bit (bitpos < 32 still)
 								s.state = ST_HEADER;
 							}
 						} else {
@@ -1131,9 +1144,18 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 			}
 
 			// (2) block headers, parsed by their own lanes
+			// (segment mode at found block starts: a header at a listed split point ends the segment; the next
+			// one starts there.  At sync points the segment ends after the empty stored block, in (3).)
 			if (s.state == ST_HEADER) {
-				int v = inf_parse_block_header(s, sm, lane, gs_lane + INF_GS_LENS);
-				if (v != LDB_SUCCESS) { s.verdict = (u32)v; s.state = ST_DONE; }
+				bool stop = false;
+				if constexpr (SEG) stop = g.any_header && inf_seg_stop(s, g, 8 * s.seg_base + inf_bits_consumed(s));
+				if (stop) {
+					s.verdict = LDB_SEG_STOPPED;
+					s.state = ST_DONE;
+				} else {
+					int v = inf_parse_block_header(s, sm, lane, gs_lane + INF_GS_LENS);
+					if (v != LDB_SUCCESS) { s.verdict = (u32)v; s.state = ST_DONE; }
+				}
 			}
 			__syncwarp();
 
@@ -1162,7 +1184,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 					u32 next = s.stored_src + len;
 					inf_bits_init(s, next);	// P = 8 * next exactly
 					if (s.is_final) { s.verdict = LDB_SUCCESS; s.state = ST_DONE; }
-					else if (SEG && len == 0 && inf_seg_stop(s, g, next)) { s.verdict = LDB_SEG_STOPPED; s.state = ST_DONE; }
+					else if (SEG && !g.any_header && len == 0 && inf_seg_stop(s, g, 8 * (s.seg_base + next))) { s.verdict = LDB_SEG_STOPPED; s.state = ST_DONE; }
 					else s.state = ST_HEADER;	// parsed in the next repetition
 				}
 			}

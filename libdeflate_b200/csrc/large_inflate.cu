@@ -3,10 +3,12 @@
 //
 // The stream is cut at its own byte-aligned sync points: every non-final empty stored block (00 00 FF FF,
 // written by zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH, pigz and compress_large) ends on a byte boundary where a
-// new block header starts.  The decode kernel's segment mode (inflate_kernel.cu) decodes every segment
-// from such a point at once; the host keeps the chain of segments that the decode from the true start
-// reaches, so every accepted byte is the serial decode's.  The kernels here are the parts around it:
+// new block header starts.  A stream without them is cut at candidate block starts found by a bit-level
+// scan.  The decode kernel's segment mode (inflate_kernel.cu) decodes every segment from such a point at
+// once; the host keeps the chain of segments that the decode from the true start reaches, so every
+// accepted byte is the serial decode's.  The kernels here are the parts around it:
 //   scan      -- every 00 00 FF FF of the input, the offsets after them in order (count + ordered write);
+//   finder    -- candidate block starts at bit offsets: dynamic-Huffman headers and stored-block ends;
 //   prefix    -- the literal stream of a segment starts with 32 KiB of window references: byte j is the
 //                low byte of symbol 256 + j (the resolve kernel then writes the LOW plane of 16-bit symbols;
 //                the high plane is resolved from the same records over a shared literal stream whose
@@ -16,6 +18,10 @@
 //   substitute-- symbol -> byte with W_{k-1}, written at out + G_k;
 //   finish    -- the ordered combine of the per-segment checksums, the trailer check and the results.
 #include "ldb_common.cuh"
+#ifdef LDB_EMU
+#include <algorithm>
+#include <string.h>
+#endif
 
 #define LI_SCAN_THREADS 256
 #define LI_SCAN_PER     256		// input bytes per thread
@@ -84,6 +90,217 @@ int ldb_launch_sync_scan_write(const u8 *in, size_t n, const u64 *d_tile_off, u6
 	LDB_CUDA_CHECK_RET(cudaGetLastError());
 	return 0;
 }
+
+// ---- block-start finder: where a stream has no sync points, candidate block starts at BIT offsets ------
+// Two kinds (DESIGN.md section 4.6):
+//   dynamic  -- a non-final dynamic-Huffman header at bit p: BFINAL 0, BTYPE 2, HLIT <= 29, HDIST <= 29, a
+//               complete precode, code lengths that decode with it without overrun or a repeat at index 0,
+//               litlen and offset codes that build_decode_table accepts, and a nonzero length for EOB;
+//   stored   -- a stored block's LEN / NLEN at byte b ends it at c = b + 4 + LEN; bit 8c is a candidate when
+//               a dynamic header as above or another stored header (BTYPE 0, LEN == ~NLEN) follows there.
+// The input is read as followed by zero bytes.  A pre-filter over every bit offset (header bits, HLIT, HDIST,
+// the precode's Kraft sum) queues survivors per CTA; the queue is then validated in full, one survivor per
+// thread.  Candidates leave through one atomic counter: the host sorts them (stored-block ends are found at
+// their LEN, not in order) and drops duplicates, so the list it uses is deterministic.  A candidate is only
+// a guess: the segment chain accepts it when the decode from the true start reaches a header exactly there.
+#define LI_BS_THREADS 256
+#define LI_BS_BYTES   4				// input bytes per thread and round: 32 bit offsets
+#define LI_BS_ROUND   (LI_BS_THREADS * LI_BS_BYTES)
+#define LI_BS_ROUNDS  64			// rounds per CTA: 64 KiB of input
+#define LI_BS_CTA     ((u64)LI_BS_ROUND * LI_BS_ROUNDS)
+
+size_t ldb_block_scan_ctas(size_t n) { return (size_t)((n + LI_BS_CTA - 1) / LI_BS_CTA); }
+
+__device__ __forceinline__ u32 li_byte(const u8 *in, size_t n, u64 i) { return i < n ? (u32)in[i] : 0u; }
+
+// 64 bits from bit o (< 64) of the 128-bit little-endian value w1:w0
+__device__ __forceinline__ u64 li_bits_at(u64 w0, u64 w1, u32 o) { return o ? (w0 >> o) | (w1 << (64 - o)) : w0; }
+
+// bit reader of the validation (rare path: byte loads)
+struct li_bitrd {
+	const u8 *in;
+	size_t n;
+	u64 p;
+	__device__ u32 get(u32 nb)
+	{
+		const u64 b = p >> 3;
+		const u32 sh = (u32)(p & 7);
+		u32 w = 0;
+		for (u32 k = 0; k < 3; k++) w |= li_byte(in, n, b + k) << (8 * k);
+		p += nb;
+		return (w >> sh) & ((1u << nb) - 1);		// nb <= 7
+	}
+};
+
+// build_decode_table's rule (inf_build_table): complete, empty, or one codeword of length 1
+__device__ bool li_code_ok(const u32 *cnt, u32 maxlen)
+{
+	while (maxlen > 1 && cnt[maxlen] == 0) maxlen--;
+	u32 used = 0;
+	for (u32 l = 1; l <= maxlen; l++) used = (used << 1) + cnt[l];
+	if (used > (1u << maxlen)) return false;
+	if (used < (1u << maxlen)) return used == 0 || (used == (1u << (maxlen - 1)) && cnt[1] == 1);
+	return true;
+}
+
+// the full test of a non-final dynamic header at bit p
+__device__ bool li_dyn_header_ok(const u8 *in, size_t n, u64 p)
+{
+	static const u8 perm[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
+	li_bitrd rd = {in, n, p};
+	if (rd.get(3) != 4) return false;	// BFINAL 0, BTYPE 2
+	const u32 hlit = 257 + rd.get(5), hdist = 1 + rd.get(5), hclen = 4 + rd.get(4);
+	if (hlit > 286 || hdist > 30) return false;
+	u32 plen[19], pcnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+	for (u32 i = 0; i < 19; i++) plen[i] = 0;
+	for (u32 i = 0; i < hclen; i++) plen[perm[i]] = rd.get(3);
+	u32 kraft = 0;
+	for (u32 i = 0; i < 19; i++) {
+		pcnt[plen[i]]++;
+		if (plen[i]) kraft += 128u >> plen[i];
+	}
+	if (kraft != 128) return false;		// an incomplete precode never yields a block with an EOB code
+	u8 psym[19];
+	u32 offs[8];
+	offs[1] = 0;
+	for (u32 l = 1; l < 7; l++) offs[l + 1] = offs[l] + pcnt[l];
+	for (u32 s = 0; s < 19; s++)
+		if (plen[s]) psym[offs[plen[s]]++] = (u8)s;
+	u32 lcnt[16], ocnt[16];
+	for (u32 l = 0; l < 16; l++) { lcnt[l] = 0; ocnt[l] = 0; }
+	const u32 total = hlit + hdist;
+	u32 i = 0, prev = 0, eob = 0;
+	while (i < total) {
+		// canonical decode of one precode symbol, one bit at a time (the code is complete)
+		u32 code = 0, first = 0, index = 0, sym = 0;
+		for (u32 l = 1; l <= 7; l++) {
+			code |= rd.get(1);
+			if (code - first < pcnt[l]) { sym = psym[index + code - first]; break; }
+			index += pcnt[l];
+			first = (first + pcnt[l]) << 1;
+			code <<= 1;
+		}
+		u32 rep = 1, val = sym;
+		if (sym == 16) {
+			if (i == 0) return false;
+			rep = 3 + rd.get(2);
+			val = prev;
+		} else if (sym == 17) {
+			rep = 3 + rd.get(3);
+			val = 0;
+		} else if (sym == 18) {
+			rep = 11 + rd.get(7);
+			val = 0;
+		}
+		if (i + rep > total) return false;
+		if (val) {
+			const u32 nl = i >= hlit ? 0 : (i + rep <= hlit ? rep : hlit - i);
+			lcnt[val] += nl;
+			ocnt[val] += rep - nl;
+		}
+		if (i <= 256 && 256 < i + rep) eob = val;
+		prev = val;
+		i += rep;
+	}
+	return eob != 0 && li_code_ok(lcnt, 15) && li_code_ok(ocnt, 15);
+}
+
+// a stored header at bit 8c (either BFINAL): BTYPE 0, then LEN == ~NLEN at byte c + 1
+__device__ __forceinline__ bool li_stored_header_ok(const u8 *in, size_t n, u64 c)
+{
+	if (c + 5 > n || (in[c] & 6)) return false;
+	const u32 len = in[c + 1] | ((u32)in[c + 2] << 8), nlen = in[c + 3] | ((u32)in[c + 4] << 8);
+	return (len ^ nlen) == 0xffffu;
+}
+
+__device__ __forceinline__ void li_emit(unsigned long long *count, u64 *cand, u64 cap, u64 p)
+{
+	const u64 at = atomicAdd(count, 1ull);
+	if (at < cap) cand[at] = p;
+}
+
+// count: candidates found (may exceed cap; then only the first cap were written, in no particular order)
+__global__ void __launch_bounds__(LI_BS_THREADS)
+ldb_block_scan_kernel(const u8 *in, size_t n, u64 cap, unsigned long long *count, u64 *cand)
+{
+	__shared__ u32 queue[8 * LI_BS_ROUND];	// pre-filter survivors of a round: bit offsets relative to it
+	__shared__ u32 nq;
+	const u32 tid = threadIdx.x;
+	for (u32 r = 0; r < LI_BS_ROUNDS; r++) {
+		const u64 r0 = (u64)blockIdx.x * LI_BS_CTA + (u64)r * LI_BS_ROUND;
+		if (r0 >= n) break;
+		if (tid == 0) nq = 0;
+		__syncthreads();
+		const u64 b0 = r0 + (u64)tid * LI_BS_BYTES;
+		if (b0 < n) {
+			u64 w0 = 0, w1 = 0;	// input bytes b0 .. b0 + 15
+			for (u32 k = 0; k < 8; k++) {
+				w0 |= (u64)li_byte(in, n, b0 + k) << (8 * k);
+				w1 |= (u64)li_byte(in, n, b0 + 8 + k) << (8 * k);
+			}
+			for (u32 q = 0; q < 8 * LI_BS_BYTES && b0 + (q >> 3) < n; q++) {
+				const u64 h = li_bits_at(w0, w1, q);
+				if ((h & 7) != 4 || ((h >> 3) & 31) > 29 || ((h >> 8) & 31) > 29) continue;
+				const u32 hclen = 4 + (u32)((h >> 13) & 15);
+				const u64 pre = li_bits_at(w0, w1, q + 17);
+				u32 kraft = 0;
+#pragma unroll
+				for (u32 i = 0; i < 19; i++) {
+					const u32 l = (u32)(pre >> (3 * i)) & 7;
+					kraft += i < hclen && l ? 128u >> l : 0u;
+				}
+				if (kraft == 128) queue[atomicAdd(&nq, 1u)] = tid * (8 * LI_BS_BYTES) + q;
+			}
+			// stored blocks whose LEN / NLEN lie in this thread's bytes end at c = b + 4 + LEN
+			for (u32 j = 0; j < LI_BS_BYTES && b0 + j + 4 <= n; j++) {
+				const u32 x = (u32)li_bits_at(w0, w1, 8 * j);
+				if (((x ^ (x >> 16)) & 0xffffu) != 0xffffu) continue;
+				const u64 c = b0 + j + 4 + (x & 0xffffu);
+				if (c < n && (li_stored_header_ok(in, n, c) || li_dyn_header_ok(in, n, 8 * c))) li_emit(count, cand, cap, 8 * c);
+			}
+		}
+		__syncthreads();
+		const u32 m = nq;
+		for (u32 e = tid; e < m; e += LI_BS_THREADS) {
+			const u64 p = 8 * r0 + queue[e];
+			if (li_dyn_header_ok(in, n, p)) li_emit(count, cand, cap, p);
+		}
+		__syncthreads();
+	}
+}
+
+int ldb_launch_block_scan(const u8 *in, size_t n, u64 *d_count, u64 *d_cand, u64 cap, void *stream)
+{
+	const size_t ctas = ldb_block_scan_ctas(n);
+	if (!ctas) return 0;
+	LDB_LAUNCH(ldb_block_scan_kernel, dim3((unsigned)ctas), dim3(LI_BS_THREADS), 0, (cudaStream_t)stream, in, n, cap,
+		   (unsigned long long *)d_count, d_cand);
+	LDB_CUDA_CHECK_RET(cudaGetLastError());
+	return 0;
+}
+
+#ifdef LDB_EMU
+// tests only (emulator build): the sorted, distinct candidates of in[0, n); returns their number, or the raw
+// count when it exceeds cap (nothing written then)
+extern "C" __attribute__((visibility("default"))) size_t ldb_block_scan_emu(const u8 *in, size_t n, u64 *out, size_t cap)
+{
+	u64 *d = nullptr;
+	if (cudaMalloc((void **)&d, (cap + 1) * sizeof(u64)) != cudaSuccess) return ~(size_t)0;
+	d[0] = 0;
+	size_t m = ~(size_t)0;
+	if (ldb_launch_block_scan(in, n, d, d + 1, cap, nullptr) == 0) {
+		cudaDeviceSynchronize();
+		m = (size_t)d[0];
+		if (m <= cap) {
+			std::sort(d + 1, d + 1 + m);
+			m = (size_t)(std::unique(d + 1, d + 1 + m) - (d + 1));
+			memcpy(out, d + 1, m * sizeof(u64));
+		}
+	}
+	cudaFree(d);
+	return m;
+}
+#endif
 
 // ---- the window-reference prefix of the literal streams ----------------------------------------------
 __global__ void __launch_bounds__(256)

@@ -229,16 +229,18 @@ size_t ldb_inflate_scratch_bytes(const ldb_launch_cfg &cfg, size_t n);
 int ldb_launch_verify_trailer(const ldb_inflate_args &a, const u32 *d_checksums, void *stream);
 
 // ---- segment mode of the decode kernel (decompress_large, DESIGN.md section 4.6) ----------------------
-// Chunk c of the launch is a SEGMENT of one stream: it starts at byte start[c] of the whole input (0: the
+// Chunk c of the launch is a SEGMENT of one stream: it starts at BIT start[c] of the whole input (0: the
 // stream start, wrapper header parsed there) and its input runs to the end of the DEFLATE data.  Its
 // output position starts at pfx[c] (matches may reach that far before the segment), the literal stream
 // keeps pfx[c] bytes free at the front of the slot, and out_avail[c] is the room after the prefix.  The
-// lane stops after a non-final empty stored block that ends on one of the sorted split points
-// split[j], j >= split_i[c].  Tokens that do not fit the slot are counted, not written.
+// lane stops at a block header whose bit position is one of the sorted split points split[j],
+// j >= split_i[c] (sync points: only after a non-final empty stored block).  Tokens that do not fit the slot are counted, not written.  With overrun != 0 every
+// chunk but chunk 0 of the launch (whose start is known to be true) gives up once its input passes
+// split[split_i[c]] by more than overrun bits.
 #define LDB_SEG_PREFIX 32768u
 struct ldb_seg_info {
-	u64 end;		// input offset after the segment (stop: a split point; final block: after its last byte)
-	u32 verdict;		// LDB_* result, or LDB_SEG_STOPPED
+	u64 end;		// stop: the split point's bit offset; final block: the byte offset after its last byte
+	u32 verdict;		// LDB_* result, LDB_SEG_STOPPED or LDB_SEG_ABANDONED
 	u32 out_len;		// output bytes (the prefix not counted)
 	u32 reach;		// deepest match reach before the segment start (0: none)
 	u32 split_j;		// stop: index of the split point it stopped at
@@ -248,15 +250,19 @@ struct ldb_seg_info {
 	u32 pad;
 };
 #define LDB_SEG_STOPPED 16
+#define LDB_SEG_ABANDONED 17
 struct ldb_seg_args {
 	const u8 *base;		// the whole input
 	u64 in_nbytes;
-	const u64 *split;	// chosen split points, ascending
+	const u64 *split;	// chosen split points (bit offsets), ascending
 	u32 nsplit;
-	const u64 *start;	// per chunk
+	const u64 *start;	// per chunk (bit offsets)
 	const u32 *pfx;
 	const u32 *split_i;
 	ldb_seg_info *info;
+	u64 overrun;		// bits a speculative chunk may read past its next split point (0: no limit)
+	u32 any_header;		// split points are found block starts: stop at any header on one (0: sync points,
+				// stop only after a non-final empty stored block that ends on one)
 };
 int ldb_launch_inflate_seg(const ldb_inflate_args &a, const ldb_seg_args &g, const ldb_launch_cfg &cfg, void *stream);
 // resolve of the high byte plane of 16-bit symbols: every chunk reads its literals from 'lit' instead of its slot
@@ -271,6 +277,8 @@ struct ldb_chain_seg {		// one segment of the decode chain, as the propagation a
 int ldb_launch_sync_scan_count(const u8 *in, size_t n, u32 *d_counts, size_t tiles, void *stream);
 int ldb_launch_sync_scan_write(const u8 *in, size_t n, const u64 *d_tile_off, u64 *d_cand, size_t tiles, void *stream);
 size_t ldb_sync_scan_tiles(size_t n);
+size_t ldb_block_scan_ctas(size_t n);
+int ldb_launch_block_scan(const u8 *in, size_t n, u64 *d_count, u64 *d_cand, u64 cap, void *stream);
 int ldb_launch_seg_prefix_fill(u8 *const *d_lit, size_t n, void *stream);
 int ldb_launch_window_chain(const ldb_chain_seg *d_segs, size_t n, u8 *d_windows, void *stream);
 int ldb_launch_substitute(const ldb_chain_seg *d_segs, size_t n, const u8 *d_windows, void *stream);

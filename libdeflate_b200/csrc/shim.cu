@@ -1212,8 +1212,10 @@ extern "C" int libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *c
 // one large stream -> its bytes (large_inflate.cu, inflate_kernel.cu segment mode; DESIGN.md 4.6)
 // ---------------------------------------------------------------------------------
 // Minimum distance in input bytes between two split points (LIBDEFLATE_B200_LARGE_SPLIT_MIN overrides;
-// default 16 KiB, below half of what a compress_large piece compresses to), and the most segments one
-// wave decodes (LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS; the token budget bounds a wave as well).
+// default 16 KiB, below half of what a compress_large piece compresses to), the most segments one
+// wave decodes (LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS; the token budget bounds a wave as well), and how far
+// a speculative segment may read past its next split point before it gives up (LIBDEFLATE_B200_LARGE_OVERRUN,
+// default 4 MiB; real blocks are far shorter).
 static size_t ldb_env_size(const char *name, size_t dflt)
 {
 	if (const char *e = getenv(name)) {
@@ -1342,7 +1344,8 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	int rc;
 
 	// ---- 1. sync points: every 00 00 FF FF, then split points at least split_min apart ----------------
-	std::vector<u64> split;
+	// (split points and segment starts are bit offsets into the input; a sync point's is 8 x its byte)
+	std::vector<u64> split, c8;
 	{
 		const size_t tiles = ldb_sync_scan_tiles(n);
 		if (tiles) {
@@ -1369,12 +1372,45 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 				std::vector<u64> cand(total);
 				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(cand.data(), b + o_cand, total * 8, cudaMemcpyDeviceToHost, ctx->stream));
 				LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
-				const u64 dmin = ldb_env_size("LIBDEFLATE_B200_LARGE_SPLIT_MIN", 16384);
-				u64 last = 0;
-				for (u64 c : cand)
-					if (c < data_end && c - last >= dmin) { split.push_back(c); last = c; }
+				for (u64 c : cand) c8.push_back(8 * c);
 			}
 		}
+	}
+	const u64 dmin = 8 * ldb_env_size("LIBDEFLATE_B200_LARGE_SPLIT_MIN", 16384);
+	auto thin = [&] {
+		u64 last = 0;
+		for (u64 c : c8)
+			if (c < 8 * data_end && c - last >= dmin) { split.push_back(c); last = c; }
+	};
+	thin();
+	// ---- 1b. no sync split point: candidate block starts at bit offsets of the DEFLATE data ------------
+	// (not below 4 split spacings of data: two or three segments would not repay the finder, the symbol
+	// planes and the window chain)
+	bool found = false;	// split points are found block starts, not sync points
+	if (split.empty() && 8 * (u64)data_end >= 4 * dmin) {
+		found = true;
+		c8.clear();
+		const u64 cap0 = data_end / 512 + 1024;		// real blocks are tens of KiB apart; a second run takes more
+		for (u64 cap = cap0;;) {
+			rc = ldb_reserve_dev(ctx->li_scan, (cap + 1) * 8 + 256);
+			if (rc) return rc;
+			u64 *d_cnt = (u64 *)ctx->li_scan.p;
+			LDB_CUDA_CHECK_RET(cudaMemsetAsync(d_cnt, 0, 8, ctx->stream));
+			rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_block_scan(in, data_end, d_cnt, d_cnt + 1, cap, ctx->stream); });
+			if (rc) return rc;
+			u64 m = 0;
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(&m, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
+			LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+			if (m > cap) { cap = m; continue; }
+			c8.resize(m);
+			if (m) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(c8.data(), d_cnt + 1, m * 8, cudaMemcpyDeviceToHost, ctx->stream));
+			LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+			break;
+		}
+		// (stored-block ends are found at their LEN, out of order)
+		std::sort(c8.begin(), c8.end());
+		c8.erase(std::unique(c8.begin(), c8.end()), c8.end());
+		thin();
 	}
 	const size_t nseg = split.size() + 1;
 	// the split list lives at the start of li_scan for the whole call
@@ -1388,6 +1424,7 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	g0.in_nbytes = n;
 	g0.split = (const u64 *)ctx->li_scan.p;
 	g0.nsplit = (u32)split.size();
+	g0.any_header = found;
 	auto seg_start = [&](size_t k) -> u64 { return k ? split[k - 1] : 0; };
 	auto seg_desc = [&](size_t k, u32 pfx, size_t room) {
 		li_seg_desc d;
@@ -1395,8 +1432,8 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		d.pfx = pfx;
 		d.split_i = (u32)(k ? k : 0);
 		d.room = room;
-		const u64 hint_end = k + 1 < nseg ? split[k] : n;
-		d.slot = align_up(pfx + ldb_inflate_tok_cap(hint_end - d.start, out_avail) + 64, 16);
+		const u64 hint_end = k + 1 < nseg ? split[k] : 8 * (u64)n;
+		d.slot = align_up(pfx + ldb_inflate_tok_cap((hint_end - d.start + 7) >> 3, out_avail) + 64, 16);
 		return d;
 	};
 
@@ -1407,6 +1444,8 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	v.result = -1;
 	const u64 budget = ldb_token_budget();
 	const size_t wave_max = ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS", (size_t)1 << 20);
+	// (found block starts only: a stream split at sync points keeps the uncapped decode it always had)
+	const u64 overrun = found ? 8 * (u64)ldb_env_size("LIBDEFLATE_B200_LARGE_OVERRUN", (size_t)4 << 20) : 0;
 	u64 G = 0;
 	size_t cur = 0;		// the next chain segment
 	rc = ldb_reserve_dev(ctx->li_carry, LDB_SEG_PREFIX);
@@ -1452,7 +1491,9 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		u8 *arr = (u8 *)ctx->li_arr.p;
 		ldb_inflate_args a;
 		ldb_seg_info *d_info;
-		rc = li_decode(ctx, format, g0, segs, arr, (u8 *)ctx->token_scratch.p, &a, &d_info);
+		ldb_seg_args gw = g0;	// speculative segments of the wave may give up past their next split point
+		gw.overrun = overrun;
+		rc = li_decode(ctx, format, gw, segs, arr, (u8 *)ctx->token_scratch.p, &a, &d_info);
 		if (rc) return rc;
 		std::vector<ldb_seg_info> info(w);
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(info.data(), d_info, w * sizeof(ldb_seg_info), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1465,10 +1506,11 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		for (;;) {
 			const ldb_seg_info &r = info[j];
 			const size_t k = k0 + j;
+			if (r.verdict == LDB_SEG_ABANDONED) { cur = k; break; }	// the next wave starts with it, uncapped
 			const bool ok = r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED;
 			if (!ok || r.reach > G || r.out_len > out_avail - G) {
 				// the segment's own limits: its input and output positions are 32-bit
-				if (data_end - seg_start(k) > 0xfffffff0u && r.verdict != LDB_SEG_STOPPED)
+				if (data_end - (seg_start(k) >> 3) > 0xfffffff0u && r.verdict != LDB_SEG_STOPPED)
 					return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment has more than 4 GiB - 16 of input", __FILE__, __LINE__);
 				if (r.verdict == LDB_INSUFFICIENT_SPACE && out_avail > 0xfffffff0u - segs[j].pfx)
 					return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment has more than 4 GiB - 32 KiB of output", __FILE__, __LINE__);

@@ -76,9 +76,10 @@ def decompress_members(api, data):
 
 
 def decompress_members_large(ctx, data):
-    """Any multi-member gzip file, each member through decompress_large: a member with sync points (zlib /
-    pigz flushes, compress_large) is decoded by the whole GPU, one without them on one lane.  Same output
-    loop as decompress_members()."""
+    """Any multi-member gzip file, each member through decompress_large: a member is decoded by the whole GPU,
+    split at its sync points (zlib / pigz flushes, compress_large) or else at the block starts a bit-level scan
+    finds (plain gzip / zlib output); only a member with neither is one lane.  Same output loop as
+    decompress_members()."""
     out, pos = [], 0
     while pos < len(data):
         avail = max(4 * (len(data) - pos), 1 << 16)

@@ -11,7 +11,10 @@ Reported, with the card's name and power limit read in the same run:
   * the same bytes as BGZF through bgzf_decompress (a host call: staging over PCIe included) and as a batch of
     64 KiB gzip chunks through decompress_batch (CUDA-event time);
   * the classic one-lane call (libdeflate_gzip_decompress) on the compress_large stream of a 16 MiB PREFIX;
-  * Python-zlib streams sync-flushed every 128 KiB and every 1 MiB (--zlib-mib MiB of class T).
+  * Python-zlib streams sync-flushed every 128 KiB and every 1 MiB (--zlib-mib MiB of class T);
+  * Python-zlib streams WITHOUT sync points (split at the block starts the finder lists): class T at L1, L6 and
+    L9 and classes M and R at L6, --zlib-mib MiB each, with the finder's own kernel time (torch.profiler, one
+    more call) and the one-lane call on the first 16 MiB of class T at L6.
 """
 import argparse
 import ctypes
@@ -134,6 +137,69 @@ def classic_prefix(ctx, host):
     return m / dt / 1e9
 
 
+def kernel_ms(fn):
+    """{kernel name: ms} of one call, from torch.profiler's CUDA activities (None where unavailable)."""
+    try:
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+        torch.cuda.init()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+        out = {}
+        for e in prof.events():
+            t = getattr(e, "device_time_total", None)
+            if t is None:
+                t = getattr(e, "cuda_time_total", 0)
+            if t:
+                out[e.name] = out.get(e.name, 0.0) + t / 1000.0
+        return out
+    except Exception as ex:  # noqa: BLE001
+        print("torch.profiler unavailable: %s" % ex, flush=True)
+        return None
+
+
+def nosync(ctx, hb, level, reps):
+    """decompress_large of a Python-zlib gzip stream without sync points."""
+    z = zlib.compressobj(level, zlib.DEFLATED, 31)
+    z = z.compress(hb) + z.flush()
+    assert b"\x00\x00\xff\xff" not in z
+    dz = Dev(ctx, len(z))
+    ctx._check(ctx.l.libdeflate_b200_memcpy_h2d(ctx.h, dz.p, z, len(z)), "h2d")
+    ctx.sync()
+    gbs, segs, stages = large(ctx, dz.p, len(z), len(hb), reps)
+    out, res = Dev(ctx, len(hb)), Dev(ctx, 32)
+    km = kernel_ms(lambda: (ctx.l.libdeflate_b200_decompress_large(ctx.h, GZ, 0, dz.p, len(z), out.p, len(hb), res.p, res.p + 8,
+                                                                    res.p + 16), ctx.sync()))
+    out.free()
+    res.free()
+    dz.free()
+    row = {"ratio": round(len(z) / len(hb), 5), "decompress_large_GB/s": round(gbs, 2), "segments": segs, "stage_ms": stages}
+    if km is not None:
+        row["finder_ms"] = round(sum(v for k, v in km.items() if "block_scan" in k), 3)
+        row["window_chain_ms"] = round(sum(v for k, v in km.items() if "window_chain" in k), 3)
+    return row
+
+
+def one_lane(ctx, hb, level):
+    """libdeflate_gzip_decompress (one lane) on a Python-zlib stream without sync points: output GB/s."""
+    l = ctx.l
+    z = zlib.compressobj(level, zlib.DEFLATED, 31)
+    z = z.compress(hb) + z.flush()
+    dz, dout = Dev(ctx, len(z)), Dev(ctx, len(hb))
+    ctx._check(l.libdeflate_b200_memcpy_h2d(ctx.h, dz.p, z, len(z)), "h2d")
+    ctx.sync()
+    d = l.libdeflate_alloc_decompressor()
+    aout = ctypes.c_size_t(0)
+    t = time.perf_counter()
+    r = l.libdeflate_gzip_decompress(d, dz.p, len(z), dout.p, len(hb), ctypes.byref(aout))
+    dt = time.perf_counter() - t
+    l.libdeflate_free_decompressor(d)
+    dz.free()
+    dout.free()
+    assert r == 0 and aout.value == len(hb)
+    return len(hb) / dt / 1e9
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mib", type=int, default=1024)
@@ -141,13 +207,23 @@ def main():
     ap.add_argument("--classes", default="T,M,R")
     ap.add_argument("--zlib-mib", type=int, default=256)
     ap.add_argument("--out", default=None, help="directory for the JSON result")
+    ap.add_argument("--nosync-only", action="store_true", help="only the streams without sync points")
     args = ap.parse_args()
     n = args.mib << 20
     name, power = card()
     res = {"card": name, "power_limit": power, "input_mib": args.mib, "format": "gzip", "level": 6, "classes": {}}
     print("card: %s, power limit %s; %d MiB per class, gzip L6" % (name, power, args.mib), flush=True)
     ctx = ldb.Context(0)
-    for cname in args.classes.split(","):
+    res["zlib_no_sync"] = {}
+    m = args.zlib_mib << 20
+    for cname, level in (("T", 1), ("T", 6), ("T", 9), ("M", 6), ("R", 6)):
+        hb = synth(m, CLASSES[cname]).tobytes()
+        row = nosync(ctx, hb, level, args.reps)
+        if (cname, level) == ("T", 6):
+            row["one_lane_16MiB_GB/s"] = round(one_lane(ctx, hb[:16 << 20], level), 4)
+        res["zlib_no_sync"]["%s_L%d" % (cname, level)] = row
+        print("zlib without sync points, class %s L%d, %d MiB: %s" % (cname, level, args.zlib_mib, json.dumps(row)), flush=True)
+    for cname in ([] if args.nosync_only else args.classes.split(",")):
         host = synth(n, CLASSES[cname])
         hb = host.tobytes()
         z = ctx.compress_large(hb, 6, GZ)
@@ -166,10 +242,9 @@ def main():
         row["classic_one_lane_16MiB_prefix_GB/s"] = round(classic_prefix(ctx, host), 4)
         res["classes"][cname] = row
         print("class %s: %s" % (cname, json.dumps(row)), flush=True)
-    m = args.zlib_mib << 20
     hb = synth(m, 0).tobytes()
     res["zlib_sync_flush"] = {}
-    for every in (128 << 10, 1 << 20):
+    for every in (() if args.nosync_only else (128 << 10, 1 << 20)):
         co = zlib.compressobj(6, zlib.DEFLATED, 31)
         z = b"".join(co.compress(hb[i:i + every]) + co.flush(zlib.Z_SYNC_FLUSH) for i in range(0, m, every)) + co.flush()
         dz = Dev(ctx, len(z))
