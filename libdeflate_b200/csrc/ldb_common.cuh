@@ -115,9 +115,9 @@ __device__ __forceinline__ u32 def_write_trailer(u8 *out, int format, u32 checks
 // Adler-32 modulus (ref: lib/adler32.c:31)
 #define LDB_ADLER_MOD  65521u
 
-// ---- checksum combine (compress_large's stitch, decompress_large's trailer check) -------------------
+// ---- checksum combine (compress_large's stitch, decompress_large's trailer check, the classic checksums) --
 // CRC-32 (reflected): a * b mod G
-__device__ __forceinline__ u32 ldb_mulmodp(u32 a, u32 b)
+__host__ __device__ __forceinline__ u32 ldb_mulmodp(u32 a, u32 b)
 {
 	u32 p = 0;
 	for (int i = 0; i < 32; i++) {
@@ -131,7 +131,7 @@ __device__ __forceinline__ u32 ldb_mulmodp(u32 a, u32 b)
 // checksum of A || B from those of A and B (len_b = |B|): CRC-32 is linear, crc(A || B) =
 // crc(A) * x^(8 len_b) + crc(B), with x^(8 * 2^i) mod G in xp[i]; Adler-32 by the zlib rule.
 // (init, 0) is the identity on both sides.
-__device__ __forceinline__ u32 ldb_sum_combine(int format, const u32 *xp, u32 a, u32 b, u64 len_b)
+__host__ __device__ __forceinline__ u32 ldb_sum_combine(int format, const u32 *xp, u32 a, u32 b, u64 len_b)
 {
 	if (format == LDB_FMT_GZIP) {
 		u32 m = 0x80000000u;	// x^0
@@ -159,19 +159,11 @@ struct ldb_crc_tables {
 	u32 lane_mult[32];	// x^(128*l) mod G for l = 0..31 (reflected representation)
 };
 
-#ifndef LDB_EMU
 #define LDB_CUDA_CHECK_RET(expr)                                                     \
 	do {                                                                         \
 		cudaError_t e__ = (expr);                                            \
 		if (e__ != cudaSuccess) return ldb_fail(e__, #expr, __FILE__, __LINE__); \
 	} while (0)
-#else
-#define LDB_CUDA_CHECK_RET(expr)                                                     \
-	do {                                                                         \
-		cudaError_t e__ = (expr);                                            \
-		if (e__ != cudaSuccess) return ldb_fail(e__, #expr, __FILE__, __LINE__); \
-	} while (0)
-#endif
 
 int ldb_fail(int err, const char *what, const char *file, int line);
 

@@ -46,25 +46,14 @@ extern "C" const char *libdeflate_b200_last_error(void) { return g_last_error; }
 // CRC-32 constant tables (host; the math follows scripts/gen-crc32-consts.py:41-86
 // and lib/crc32.c:76-100 but the table shapes are the kernel's own)
 // ---------------------------------------------------------------------------------
-static u32 h_multmodp(u32 a, u32 b)
-{
-	u32 p = 0;
-	for (int i = 0; i < 32; i++) {
-		if (a & 0x80000000u) p ^= b;
-		a <<= 1;
-		b = (b >> 1) ^ ((b & 1) ? LDB_CRC32_POLY : 0);
-	}
-	return p;
-}
-
 // x^(8*nbytes) mod G
 static u32 h_xpow8(u64 nbytes)
 {
 	u32 result = 0x80000000u;	// x^0
 	u32 sq = 0x00800000u;		// x^8
 	while (nbytes) {
-		if (nbytes & 1) result = h_multmodp(sq, result);
-		sq = h_multmodp(sq, sq);
+		if (nbytes & 1) result = ldb_mulmodp(sq, result);
+		sq = ldb_mulmodp(sq, sq);
 		nbytes >>= 1;
 	}
 	return result;
@@ -85,24 +74,8 @@ static void ldb_build_crc_tables(ldb_crc_tables *t)
 	const u32 x512 = h_xpow8(512);
 	for (int j = 0; j < 4; j++)
 		for (u32 b = 0; b < 256; b++)
-			t->fold512[j][b] = h_multmodp(x512, b << (8 * j));
+			t->fold512[j][b] = ldb_mulmodp(x512, b << (8 * j));
 	for (u32 l = 0; l < 32; l++) t->lane_mult[l] = h_xpow8(16 * l);
-}
-
-static u32 h_crc32_combine(u32 crc1, u32 crc2, u64 len2) { return h_multmodp(h_xpow8(len2), crc1) ^ crc2; }
-
-static u32 h_adler32_combine(u32 a1, u32 a2, u64 len2)
-{
-	const u32 M = LDB_ADLER_MOD;
-	u32 rem = (u32)(len2 % M);
-	u32 s1 = a1 & 0xffff, s2 = (u32)(((u64)rem * s1) % M);
-	s1 += (a2 & 0xffff) + M - 1;
-	s2 += (a1 >> 16) + (a2 >> 16) + M - rem;
-	if (s1 >= M) s1 -= M;
-	if (s1 >= M) s1 -= M;
-	if (s2 >= (M << 1)) s2 -= (M << 1);
-	if (s2 >= M) s2 -= M;
-	return s1 | (s2 << 16);
 }
 
 // ---------------------------------------------------------------------------------
@@ -296,7 +269,8 @@ template <typename F> static int ldb_timed_launch(libdeflate_b200_ctx *ctx, int 
 extern "C" void libdeflate_b200_ctx_set_profiling(struct libdeflate_b200_ctx *ctx, int on) { ctx->profiling = on; }
 
 // Sum of device time (ms) and number of launches of one kernel kind since the last reset;
-// synchronises the stream.  kind: 0 crc32, 1 adler32, 2 inflate (decode), 3 verify, 4 deflate, 5 inflate (resolve).
+// synchronises the stream.  kind: 0 crc32, 1 adler32, 2 inflate (decode), 3 verify, 4 deflate, 5 inflate (resolve),
+// 6 pack (the packing, large-stream stitch, scan and window kernels).
 extern "C" double libdeflate_b200_kernel_time_ms(struct libdeflate_b200_ctx *ctx, int kind, uint64_t *n_launches)
 {
 	cudaStreamSynchronize(ctx->stream);
@@ -388,6 +362,42 @@ struct host_scratch {
 	host_scratch &operator=(const host_scratch &) = delete;
 };
 
+static int check_format(int format)
+{
+	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
+	return 0;
+}
+
+// -1 selects the default level, 6
+static int check_level(int *level)
+{
+	if (*level == -1) *level = 6;
+	if (*level < 0 || *level > 12) return ldb_fail(cudaErrorInvalidValue, "level", __FILE__, __LINE__);
+	return 0;
+}
+
+// bytes the zlib / gzip wrapper adds to a raw DEFLATE stream
+static size_t wrap_bytes(int format) { return format == LDB_FMT_GZIP ? 18 : (format == LDB_FMT_ZLIB ? 6 : 0); }
+
+// a positive integer from the environment; dflt when the variable is unset or not positive
+static size_t ldb_env_size(const char *name, size_t dflt)
+{
+	if (const char *e = getenv(name)) {
+		long long v = atoll(e);
+		if (v > 0) return (size_t)v;
+	}
+	return dflt;
+}
+
+// CRC-32 (gzip) or Adler-32 (zlib) of n device buffers into sums; nothing for raw DEFLATE
+static int launch_checksum(libdeflate_b200_ctx *ctx, int format, const void *const *ptrs, const size_t *lens, u32 *sums, size_t n)
+{
+	if (format == LDB_FMT_GZIP)
+		return ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, ptrs, lens, nullptr, sums, n, ctx->cfg, ctx->stream); });
+	if (format == LDB_FMT_ZLIB)
+		return ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32(ptrs, lens, nullptr, sums, n, ctx->cfg, ctx->stream); });
+	return 0;
+}
 
 extern "C" int libdeflate_b200_crc32_batch(struct libdeflate_b200_ctx *ctx, const void *const *d_ptrs,
 					    const size_t *d_nbytes, const uint32_t *d_init,
@@ -412,15 +422,7 @@ extern "C" int libdeflate_b200_adler32_batch(struct libdeflate_b200_ctx *ctx, co
 // depend on in_nbytes / out_avail, which live in device memory: when the caller cannot give the
 // host copies (h_in_nbytes / h_out_avail, as the *_host entry points can), the prefix sums are
 // computed on the device and read back -- the one place where this call waits for the stream.
-static size_t ldb_token_budget(void)
-{
-	size_t mb = 8192;
-	if (const char *e = getenv("LIBDEFLATE_B200_TOKEN_BUDGET_MB")) {
-		long v = atol(e);
-		if (v > 0) mb = (size_t)v;
-	}
-	return mb << 20;
-}
+static u64 token_budget_bytes(void) { return (u64)ldb_env_size("LIBDEFLATE_B200_TOKEN_BUDGET_MB", 8192) << 20; }
 
 static int ldb_decompress_batch_impl(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
 				     const void *const *d_in_ptrs, const size_t *d_in_nbytes,
@@ -430,9 +432,10 @@ static int ldb_decompress_batch_impl(struct libdeflate_b200_ctx *ctx, int format
 				     const size_t *h_in_nbytes, const size_t *h_out_avail)
 {
 	if (n == 0) return 0;
-	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
+	int rc = check_format(format);
+	if (rc) return rc;
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
-	int rc = ldb_reserve_dev(ctx->inflate_scratch, ldb_inflate_scratch_bytes(ctx->cfg, n));
+	rc = ldb_reserve_dev(ctx->inflate_scratch, ldb_inflate_scratch_bytes(ctx->cfg, n));
 	if (rc) return rc;
 	// tmp layout: actual_out scratch (size_t[n]) | trailer u32[n] | isize u32[n] | checksums u32[n]
 	//             | token counts u32[2n] | token slot offsets u64[n + 1]
@@ -491,38 +494,34 @@ static int ldb_decompress_batch_impl(struct libdeflate_b200_ctx *ctx, int format
 	a.format = format;
 	a.flags = flags;
 
-	// waves
-	const u64 budget = ldb_token_budget();
+	// waves: chunks [wave[k], wave[k + 1]), each as long as its slots fit the budget (at least one chunk)
+	const u64 budget = token_budget_bytes();
+	std::vector<size_t> wave(1, 0);
 	u64 need = 0;
 	for (size_t i0 = 0; i0 < n;) {
 		size_t i1 = i0 + 1;
 		while (i1 < n && h_off[i1 + 1] - h_off[i0] <= budget) i1++;
 		if (h_off[i1] - h_off[i0] > need) need = h_off[i1] - h_off[i0];
+		wave.push_back(i1);
 		i0 = i1;
 	}
 	rc = ldb_reserve_dev(ctx->token_scratch, (size_t)need + 256);
 	if (rc) return rc;
 	a.tok_base = (u8 *)ctx->token_scratch.p;
-	for (size_t i0 = 0; i0 < n;) {
-		size_t i1 = i0 + 1;
-		while (i1 < n && h_off[i1 + 1] - h_off[i0] <= budget) i1++;
-		a.first = i0;
-		a.count = i1 - i0;
-		a.tok_origin = h_off[i0];
+	for (size_t k = 0; k + 1 < wave.size(); k++) {
+		a.first = wave[k];
+		a.count = wave[k + 1] - wave[k];
+		a.tok_origin = h_off[wave[k]];
 		rc = ldb_timed_launch(ctx, LDB_K_INFLATE, [&] { return ldb_launch_inflate(a, ctx->cfg, ctx->stream); });
 		if (rc) return rc;
 		rc = ldb_timed_launch(ctx, LDB_K_RESOLVE, [&] { return ldb_launch_inflate_resolve(a, ctx->cfg, ctx->stream); });
 		if (rc) return rc;
-		i0 = i1;
 	}
 	a.first = 0;
 	a.count = n;
 	if (format != LDB_FMT_RAW) {
 		// checksum of what was produced, then compare with the trailer
-		if (format == LDB_FMT_GZIP)
-			rc = ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, (const void *const *)d_out_ptrs, a.actual_out, nullptr, sums, n, ctx->cfg, ctx->stream); });
-		else
-			rc = ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32((const void *const *)d_out_ptrs, a.actual_out, nullptr, sums, n, ctx->cfg, ctx->stream); });
+		rc = launch_checksum(ctx, format, (const void *const *)d_out_ptrs, a.actual_out, sums, n);
 		if (rc) return rc;
 		rc = ldb_timed_launch(ctx, LDB_K_VERIFY, [&] { return ldb_launch_verify_trailer(a, sums, ctx->stream); });
 	}
@@ -545,19 +544,16 @@ extern "C" int libdeflate_b200_compress_batch(struct libdeflate_b200_ctx *ctx, i
 					       size_t *d_out_nbytes, size_t n)
 {
 	if (n == 0) return 0;
-	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
-	if (level == -1) level = 6;
-	if (level < 0 || level > 12) return ldb_fail(cudaErrorInvalidValue, "level", __FILE__, __LINE__);
+	int rc = check_format(format);
+	if (!rc) rc = check_level(&level);
+	if (rc) return rc;
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
-	int rc = ldb_reserve_dev(ctx->deflate_scratch, ldb_deflate_scratch_bytes(ctx->cfg, n));
+	rc = ldb_reserve_dev(ctx->deflate_scratch, ldb_deflate_scratch_bytes(ctx->cfg, n));
 	if (rc) return rc;
 	rc = ldb_reserve_dev(ctx->tmp, align_up(n * sizeof(u32), 256));
 	if (rc) return rc;
 	u32 *sums = (u32 *)ctx->tmp.p;
-	if (format == LDB_FMT_GZIP)
-		rc = ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, d_in_ptrs, d_in_nbytes, nullptr, sums, n, ctx->cfg, ctx->stream); });
-	else if (format == LDB_FMT_ZLIB)
-		rc = ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32(d_in_ptrs, d_in_nbytes, nullptr, sums, n, ctx->cfg, ctx->stream); });
+	rc = launch_checksum(ctx, format, d_in_ptrs, d_in_nbytes, sums, n);
 	if (rc) return rc;
 	ldb_deflate_args a;
 	a.in_ptrs = d_in_ptrs;
@@ -633,7 +629,7 @@ struct staged_batch {
 	size_t *d_sizes;	// device array
 	u8 *d_base;		// device slab
 	std::size_t slab_bytes;
-	bool compact;
+	host_span span;		// of the host buffers; compact: mirrored in the slab at its 16-byte phase
 	size_t *offsets;	// host, per chunk offset into slab (malloc'd, owned)
 	~staged_batch() { free(offsets); }
 };
@@ -643,7 +639,7 @@ static int stage_layout(libdeflate_b200_ctx *ctx, ldb_buf &slab, const void *con
 			size_t n, bool copy_in, bool exact, u8 *param_base_d, u8 *param_base_h, staged_batch *sb, bool one_alloc = false)
 {
 	host_span sp = span_of(h_ptrs, h_sizes, n, exact, one_alloc);
-	sb->compact = sp.compact;
+	sb->span = sp;
 	sb->offsets = (size_t *)malloc(n * sizeof(size_t) + 8);
 	size_t total = 0;
 	if (sp.compact) {
@@ -706,20 +702,23 @@ static bool host_ordered(const void *const *ptrs, const size_t *sizes, size_t n)
 	return n && ptrs[n - 1];
 }
 
+// h_out NULL: the outputs do not go to caller buffers (the packed compress form)
 static bool pipeline_eligible(const libdeflate_b200_ctx *ctx, const void *const *h_in, const size_t *in_sz,
 			      const void *const *h_out, const size_t *out_sz, size_t n, bool in_one_alloc = false)
 {
 	if (n < LDB_PIPE_MIN_CHUNKS || !ctx->stream_h2d || !ctx->stream_d2h) return false;
 	if (getenv("LIBDEFLATE_B200_NO_PIPELINE")) return false;
-	host_span a = span_of(h_in, in_sz, n, false, in_one_alloc), b = span_of(h_out, out_sz, n, true);
-	return a.compact && b.compact && host_ordered(h_in, in_sz, n) && host_ordered(h_out, out_sz, n);
+	if (!span_of(h_in, in_sz, n, false, in_one_alloc).compact || !host_ordered(h_in, in_sz, n)) return false;
+	return !h_out || (span_of(h_out, out_sz, n, true).compact && host_ordered(h_out, out_sz, n));
 }
 
-static void pipe_events_destroy(struct pipe_events *e);
 struct pipe_events {
 	cudaEvent_t in[LDB_PIPE_MAX_STAGES], done[LDB_PIPE_MAX_STAGES];
 	int n = 0;
-	~pipe_events() { pipe_events_destroy(this); }
+	~pipe_events()
+	{
+		for (int i = 0; i < n; i++) { cudaEventDestroy(in[i]); cudaEventDestroy(done[i]); }
+	}
 };
 static int pipe_events_create(pipe_events *e, int n)
 {
@@ -730,11 +729,6 @@ static int pipe_events_create(pipe_events *e, int n)
 		e->n = i + 1;
 	}
 	return 0;
-}
-static void pipe_events_destroy(pipe_events *e)
-{
-	for (int i = 0; i < e->n; i++) { cudaEventDestroy(e->in[i]); cudaEventDestroy(e->done[i]); }
-	e->n = 0;
 }
 // min_chunks: smallest sub-batch that still fills the kernel of this direction (the inflate kernel
 // decodes one chunk per lane, ~71 K lanes resident; the deflate kernel one chunk per CTA)
@@ -748,6 +742,100 @@ static size_t pipe_stages(size_t n, size_t total_bytes, size_t min_chunks)
 	return s;
 }
 
+// H2D of the input bytes of sub-batch [i0, i1) into its compact slab (copy stream); the compute stream
+// waits for them through 'uploaded'.
+static int upload_sub_batch(libdeflate_b200_ctx *ctx, const staged_batch &sb, const void *const *h_in, const size_t *h_in_nbytes,
+			    size_t i0, size_t i1, cudaEvent_t uploaded)
+{
+	const u8 *ilo = (const u8 *)h_in[i0], *ihi = (const u8 *)h_in[i1 - 1] + h_in_nbytes[i1 - 1];
+	const size_t mis = (uintptr_t)sb.span.lo & 15;
+	if (ihi > ilo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(sb.d_base + mis + (ilo - sb.span.lo), ilo, (size_t)(ihi - ilo), cudaMemcpyHostToDevice, ctx->stream_h2d));
+	LDB_CUDA_CHECK_RET(cudaEventRecord(uploaded, ctx->stream_h2d));
+	LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream, uploaded, 0));
+	return 0;
+}
+
+// What the host-buffer batch driver needs to know about one direction.
+struct host_batch_dir {
+	size_t res_bytes;	// device result arrays, after the parameter block; read back into the caller's h_res
+	size_t min_chunks;	// of pipe_stages()
+	bool zero_out;		// clear the output slab before the kernels run
+};
+
+// The host-buffer batch driver of compress_batch_host and the decompress host forms: stages the inputs
+// and the output layout, runs run(in, out, d_res, i0, i1) -- the device batch call on chunks [i0, i1) --
+// once or pipelined in sub-batches, reads the results back into h_res and the output bytes into the
+// caller's buffers.  Outputs that tile one span travel back whole; scattered ones receive produced(i)
+// bytes per chunk, read after the results.
+template <typename Run, typename Produced>
+static int host_batch(libdeflate_b200_ctx *ctx, const host_batch_dir &dir, const void *const *h_in, const size_t *h_in_nbytes,
+		      void *const *h_out, const size_t *h_out_avail, size_t n, bool in_one_alloc, u8 *h_res,
+		      Run &&run, Produced &&produced)
+{
+	cudaSetDevice(ctx->device);
+	stream_quiesce quiesce(ctx);
+	// parameter block: in ptrs/sizes | out ptrs/sizes | results
+	const size_t pb = param_block_bytes(n);
+	int rc = ldb_reserve_dev(ctx->d_params, 2 * pb + dir.res_bytes);
+	if (rc) return rc;
+	host_scratch hparam_own(2 * pb);
+	u8 *hparam = (u8 *)hparam_own.p;
+	if (!hparam) return ldb_fail(cudaErrorMemoryAllocation, "malloc", __FILE__, __LINE__);
+	u8 *dparam = (u8 *)ctx->d_params.p, *d_res = dparam + 2 * pb;
+	const void *const *h_outc = (const void *const *)h_out;
+	const bool pipelined = pipeline_eligible(ctx, h_in, h_in_nbytes, h_outc, h_out_avail, n, in_one_alloc);
+	staged_batch in_sb{}, out_sb{};
+	rc = stage_layout(ctx, ctx->d_stage_in, h_in, h_in_nbytes, n, !pipelined, false, dparam, hparam, &in_sb, in_one_alloc);
+	if (rc) return rc;
+	rc = stage_layout(ctx, ctx->d_stage_out, h_outc, h_out_avail, n, false, true, dparam + pb, hparam + pb, &out_sb);
+	if (rc) return rc;
+	// whole output spans travel back: what the kernels do not write (room past actual_out, failed chunks) must
+	// not be bytes of an earlier call
+	if (dir.zero_out) LDB_CUDA_CHECK_RET(cudaMemsetAsync(out_sb.d_base, 0, out_sb.slab_bytes, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(dparam, hparam, 2 * pb, cudaMemcpyHostToDevice, ctx->stream));
+	const host_span osp = out_sb.span;
+	const size_t omis = (uintptr_t)osp.lo & 15;
+	if (pipelined) {
+		const size_t S = pipe_stages(n, (size_t)(in_sb.span.hi - in_sb.span.lo) + (size_t)(osp.hi - osp.lo), dir.min_chunks);
+		pipe_events ev;
+		rc = pipe_events_create(&ev, (int)S);
+		if (rc) return rc;
+		for (size_t k = 0; k < S; k++) {
+			const size_t i0 = n * k / S, i1 = n * (k + 1) / S;
+			rc = upload_sub_batch(ctx, in_sb, h_in, h_in_nbytes, i0, i1, ev.in[k]);
+			if (rc) return rc;
+			rc = run(in_sb, out_sb, d_res, i0, i1);
+			if (rc) return rc;
+			LDB_CUDA_CHECK_RET(cudaEventRecord(ev.done[k], ctx->stream));
+			LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream_d2h, ev.done[k], 0));
+			u8 *olo = (u8 *)h_out[i0], *ohi = (u8 *)h_out[i1 - 1] + h_out_avail[i1 - 1];
+			if (ohi > olo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(olo, out_sb.d_base + omis + (olo - osp.lo), (size_t)(ohi - olo), cudaMemcpyDeviceToHost, ctx->stream_d2h));
+		}
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream_d2h));
+	} else {
+		rc = run(in_sb, out_sb, d_res, 0, n);
+		if (rc) return rc;
+	}
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(h_res, d_res, dir.res_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	// output bytes back to the caller's buffers (the pipeline has done so already)
+	if (pipelined) return 0;
+	if (osp.compact) {
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)osp.lo, out_sb.d_base + omis, (size_t)(osp.hi - osp.lo), cudaMemcpyDeviceToHost, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+		return 0;
+	}
+	rc = ldb_reserve_pinned(ctx->h_pinned, out_sb.slab_bytes);
+	if (rc) return rc;
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->h_pinned.p, out_sb.d_base, out_sb.slab_bytes - 64, cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	for (size_t i = 0; i < n; i++) {
+		const size_t nb = produced(i);
+		if (nb && h_out[i]) memcpy(h_out[i], (u8 *)ctx->h_pinned.p + out_sb.offsets[i], nb);
+	}
+	return 0;
+}
+
 static int ldb_decompress_batch_host_impl(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
 					  const void *const *h_in, const size_t *h_in_nbytes,
 					  void *const *h_out, const size_t *h_out_avail,
@@ -755,91 +843,30 @@ static int ldb_decompress_batch_host_impl(struct libdeflate_b200_ctx *ctx, int f
 					  int32_t *h_results, size_t n, bool in_one_alloc)
 {
 	if (n == 0) return 0;
-	cudaSetDevice(ctx->device);
-	stream_quiesce quiesce(ctx);
-	// parameter block: in ptrs/sizes | out ptrs/sizes | actual_in | actual_out | results
-	size_t pb = param_block_bytes(n);
-	size_t res_off = 2 * pb;
-	size_t res_bytes = 2 * align_up(n * sizeof(size_t), 256) + align_up(n * sizeof(s32), 256);
-	int rc = ldb_reserve_dev(ctx->d_params, res_off + res_bytes);
+	// results: actual_in | actual_out | result
+	const size_t a8 = align_up(n * sizeof(size_t), 256);
+	const host_batch_dir dir = {2 * a8 + align_up(n * sizeof(s32), 256), 16384, true};
+	host_scratch res_own(dir.res_bytes);
+	u8 *res = (u8 *)res_own.p;
+	if (!res) return ldb_fail(cudaErrorMemoryAllocation, "malloc", __FILE__, __LINE__);
+	const size_t *r_ain = (const size_t *)res, *r_aout = (const size_t *)(res + a8);
+	const s32 *r_res = (const s32 *)(res + 2 * a8);
+	int rc = host_batch(
+		ctx, dir, h_in, h_in_nbytes, h_out, h_out_avail, n, in_one_alloc, res,
+		[&](const staged_batch &in, const staged_batch &out, u8 *d_res, size_t i0, size_t i1) {
+			return ldb_decompress_batch_impl(ctx, format, flags, (const void *const *)in.d_ptrs + i0, in.d_sizes + i0,
+							 (void *const *)out.d_ptrs + i0, out.d_sizes + i0, (size_t *)d_res + i0,
+							 (size_t *)(d_res + a8) + i0, (s32 *)(d_res + 2 * a8) + i0, i1 - i0,
+							 h_in_nbytes + i0, h_out_avail + i0);
+		},
+		[&](size_t i) -> size_t { return r_res[i] == LDB_SUCCESS || r_res[i] == LDB_SHORT_OUTPUT ? r_aout[i] : 0; });
 	if (rc) return rc;
-	host_scratch hparam_own(res_off + res_bytes);
-	u8 *hparam = (u8 *)hparam_own.p;
-	if (!hparam) return ldb_fail(cudaErrorMemoryAllocation, "malloc", __FILE__, __LINE__);
-	u8 *dparam = (u8 *)ctx->d_params.p;
-	const bool pipelined = pipeline_eligible(ctx, h_in, h_in_nbytes, (const void *const *)h_out, h_out_avail, n, in_one_alloc);
-	staged_batch in_sb{}, out_sb{};
-	rc = stage_layout(ctx, ctx->d_stage_in, h_in, h_in_nbytes, n, !pipelined, false, dparam, hparam, &in_sb, in_one_alloc);
-	if (!rc) rc = stage_layout(ctx, ctx->d_stage_out, (const void *const *)h_out, h_out_avail, n, false, true, dparam + pb, hparam + pb, &out_sb);
-	// whole output spans travel back: what the kernels do not write (room past actual_out, failed chunks) must
-	// not be bytes of an earlier call
-	if (!rc) rc = cudaMemsetAsync(out_sb.d_base, 0, out_sb.slab_bytes, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "memset out", __FILE__, __LINE__);
-	if (!rc) rc = cudaMemcpyAsync(dparam, hparam, 2 * pb, cudaMemcpyHostToDevice, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "H2D params", __FILE__, __LINE__);
-	size_t *d_ain = (size_t *)(dparam + res_off);
-	size_t *d_aout = (size_t *)(dparam + res_off + align_up(n * sizeof(size_t), 256));
-	s32 *d_res = (s32 *)(dparam + res_off + 2 * align_up(n * sizeof(size_t), 256));
-	bool out_copied = false;
-	if (!rc && pipelined) {
-		host_span isp = span_of(h_in, h_in_nbytes, n, false, in_one_alloc), osp = span_of((const void *const *)h_out, h_out_avail, n, true);
-		const size_t imis = (uintptr_t)isp.lo & 15, omis = (uintptr_t)osp.lo & 15;
-		const size_t S = pipe_stages(n, (size_t)(isp.hi - isp.lo) + (size_t)(osp.hi - osp.lo), 16384);
-		pipe_events ev;
-		rc = pipe_events_create(&ev, (int)S);
-		for (size_t k = 0; k < S && !rc; k++) {
-			const size_t i0 = n * k / S, i1 = n * (k + 1) / S;
-			const u8 *ilo = (const u8 *)h_in[i0], *ihi = (const u8 *)h_in[i1 - 1] + h_in_nbytes[i1 - 1];
-			u8 *olo = (u8 *)h_out[i0], *ohi = (u8 *)h_out[i1 - 1] + h_out_avail[i1 - 1];
-			if (ihi > ilo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(in_sb.d_base + imis + (ilo - isp.lo), ilo, (size_t)(ihi - ilo), cudaMemcpyHostToDevice, ctx->stream_h2d));
-			LDB_CUDA_CHECK_RET(cudaEventRecord(ev.in[k], ctx->stream_h2d));
-			LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream, ev.in[k], 0));
-			rc = ldb_decompress_batch_impl(ctx, format, flags, (const void *const *)in_sb.d_ptrs + i0, in_sb.d_sizes + i0,
-						       (void *const *)out_sb.d_ptrs + i0, out_sb.d_sizes + i0, d_ain + i0, d_aout + i0, d_res + i0, i1 - i0,
-						       h_in_nbytes + i0, h_out_avail + i0);
-			if (rc) break;
-			LDB_CUDA_CHECK_RET(cudaEventRecord(ev.done[k], ctx->stream));
-			LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream_d2h, ev.done[k], 0));
-			if (ohi > olo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(olo, out_sb.d_base + omis + (olo - osp.lo), (size_t)(ohi - olo), cudaMemcpyDeviceToHost, ctx->stream_d2h));
-		}
-		if (!rc) rc = cudaStreamSynchronize(ctx->stream_d2h) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync d2h", __FILE__, __LINE__);
-		pipe_events_destroy(&ev);
-		out_copied = true;
-	} else if (!rc) {
-		rc = ldb_decompress_batch_impl(ctx, format, flags, (const void *const *)in_sb.d_ptrs, in_sb.d_sizes,
-					       (void *const *)out_sb.d_ptrs, out_sb.d_sizes, d_ain, d_aout, d_res, n, h_in_nbytes, h_out_avail);
+	for (size_t i = 0; i < n; i++) {
+		if (h_results) h_results[i] = r_res[i];
+		if (h_actual_in) h_actual_in[i] = r_ain[i];
+		if (h_actual_out) h_actual_out[i] = r_aout[i];
 	}
-	u8 *hres = hparam + res_off;
-	if (!rc) rc = cudaMemcpyAsync(hres, dparam + res_off, res_bytes, cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "D2H results", __FILE__, __LINE__);
-	if (!rc) rc = cudaStreamSynchronize(ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-	if (!rc) {
-		const size_t *r_ain = (const size_t *)hres;
-		const size_t *r_aout = (const size_t *)(hres + align_up(n * sizeof(size_t), 256));
-		const s32 *r_res = (const s32 *)(hres + 2 * align_up(n * sizeof(size_t), 256));
-		// output bytes back to the caller's buffers
-		if (out_copied) {
-			// done by the pipeline
-		} else if (out_sb.compact) {
-			host_span sp = span_of((const void *const *)h_out, h_out_avail, n, true);
-			size_t mis = (uintptr_t)sp.lo & 15;
-			if (sp.lo)
-				rc = cudaMemcpyAsync((void *)sp.lo, out_sb.d_base + mis, (size_t)(sp.hi - sp.lo), cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "D2H out", __FILE__, __LINE__);
-		} else {
-			rc = ldb_reserve_pinned(ctx->h_pinned, out_sb.slab_bytes);
-			if (!rc) rc = cudaMemcpyAsync(ctx->h_pinned.p, out_sb.d_base, out_sb.slab_bytes - 64, cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "D2H out", __FILE__, __LINE__);
-			if (!rc) rc = cudaStreamSynchronize(ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-			if (!rc)
-				for (size_t i = 0; i < n; i++) {
-					size_t nb = (r_res[i] == LDB_SUCCESS || r_res[i] == LDB_SHORT_OUTPUT) ? r_aout[i] : 0;
-					if (nb && h_out[i]) memcpy(h_out[i], (u8 *)ctx->h_pinned.p + out_sb.offsets[i], nb);
-				}
-		}
-		if (!rc) rc = cudaStreamSynchronize(ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-		for (size_t i = 0; i < n; i++) {
-			if (h_results) h_results[i] = r_res[i];
-			if (h_actual_in) h_actual_in[i] = r_ain[i];
-			if (h_actual_out) h_actual_out[i] = r_aout[i];
-		}
-	}
-	return rc;
+	return 0;
 }
 
 extern "C" int libdeflate_b200_decompress_batch_host(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
@@ -883,13 +910,6 @@ extern "C" int libdeflate_b200_pack_batch(struct libdeflate_b200_ctx *ctx, const
 	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_pack(d_ptrs, d_sizes, n, d_dense, dense_avail, (u64 *)d_offsets, ctx->cfg, ctx->stream); });
 }
 
-static size_t bound_of(int format, size_t n)
-{
-	size_t blocks = (n + 4999) / 5000;
-	if (blocks < 1) blocks = 1;
-	return 5 * blocks + n + (format == LDB_FMT_GZIP ? 18 : (format == LDB_FMT_ZLIB ? 6 : 0));
-}
-
 // Packed output: chunk i is written to h_out + h_offsets[i] (16-byte aligned starts, h_offsets[n] =
 // bytes used), h_out_nbytes[i] = its size (0: input too large for its compress bound -- cannot
 // happen).  The batch is compressed into bound-sized device slots, packed on the device, and only
@@ -901,7 +921,8 @@ extern "C" int libdeflate_b200_compress_batch_host_packed(struct libdeflate_b200
 {
 	if (h_offsets) h_offsets[0] = 0;
 	if (n == 0) return 0;
-	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
+	int rc = check_format(format);
+	if (rc) return rc;
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
 	stream_quiesce quiesce(ctx);
 	// device slots: one per chunk, compress_bound() rounded up to 16
@@ -911,24 +932,24 @@ extern "C" int libdeflate_b200_compress_batch_host_packed(struct libdeflate_b200
 	size_t slots = 0;
 	for (size_t i = 0; i < n; i++) {
 		slot_off[i] = slots;
-		slots += align_up(bound_of(format, h_in_nbytes[i]), 16);
+		slots += align_up(wrap_bytes(format) + ldb_raw_bound(h_in_nbytes[i]), 16);
 	}
 	slot_off[n] = slots;
 	// parameter block: in ptrs/sizes | out ptrs/avail | out sizes | offsets (n + 1 u64, per sub-batch)
 	const size_t pb = param_block_bytes(n);
 	const size_t sz_off = 2 * pb, off_off = sz_off + align_up(n * sizeof(size_t), 256);
 	const size_t par_bytes = off_off + align_up((n + LDB_PIPE_MAX_STAGES + 1) * sizeof(u64), 256);
-	int rc = ldb_reserve_dev(ctx->d_params, par_bytes);
+	rc = ldb_reserve_dev(ctx->d_params, par_bytes);
 	if (rc) return rc;
 	host_scratch hparam_own(par_bytes);
 	u8 *hparam = (u8 *)hparam_own.p;
 	if (!hparam) return ldb_fail(cudaErrorMemoryAllocation, "malloc", __FILE__, __LINE__);
 	u8 *dparam = (u8 *)ctx->d_params.p;
 	rc = ldb_reserve_dev(ctx->d_stage_out, slots + 64);
-	if (!rc) rc = ldb_reserve_dev(ctx->d_pack, slots + 64);
 	if (rc) return rc;
-	const bool pipelined = n >= LDB_PIPE_MIN_CHUNKS && ctx->stream_h2d && ctx->stream_d2h && !getenv("LIBDEFLATE_B200_NO_PIPELINE") &&
-			       span_of(h_in, h_in_nbytes, n, false).compact && host_ordered(h_in, h_in_nbytes, n);
+	rc = ldb_reserve_dev(ctx->d_pack, slots + 64);
+	if (rc) return rc;
+	const bool pipelined = pipeline_eligible(ctx, h_in, h_in_nbytes, nullptr, nullptr, n);
 	staged_batch in_sb{};
 	rc = stage_layout(ctx, ctx->d_stage_in, h_in, h_in_nbytes, n, !pipelined, false, dparam, hparam, &in_sb);
 	if (rc) return rc;
@@ -954,8 +975,6 @@ extern "C" int libdeflate_b200_compress_batch_host_packed(struct libdeflate_b200
 	pipe_events ev;
 	rc = pipe_events_create(&ev, (int)S);
 	if (rc) return rc;
-	host_span isp = span_of(h_in, h_in_nbytes, n, false);
-	const size_t imis = (uintptr_t)isp.lo & 15;
 	u64 host_pos = 0;	// bytes of h_out used so far
 	bool too_small = false;
 	// sub-batch k: H2D -> compress -> pack -> offsets/sizes D2H; its packed bytes are fetched while
@@ -979,10 +998,8 @@ extern "C" int libdeflate_b200_compress_batch_host_packed(struct libdeflate_b200
 	for (size_t k = 0; k < S; k++) {
 		const size_t i0 = n * k / S, i1 = n * (k + 1) / S;
 		if (pipelined) {
-			const u8 *ilo = (const u8 *)h_in[i0], *ihi = (const u8 *)h_in[i1 - 1] + h_in_nbytes[i1 - 1];
-			if (ihi > ilo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(in_sb.d_base + imis + (ilo - isp.lo), ilo, (size_t)(ihi - ilo), cudaMemcpyHostToDevice, ctx->stream_h2d));
-			LDB_CUDA_CHECK_RET(cudaEventRecord(ev.in[k], ctx->stream_h2d));
-			LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream, ev.in[k], 0));
+			rc = upload_sub_batch(ctx, in_sb, h_in, h_in_nbytes, i0, i1, ev.in[k]);
+			if (rc) return rc;
 		}
 		rc = libdeflate_b200_compress_batch(ctx, format, level, (const void *const *)in_sb.d_ptrs + i0, in_sb.d_sizes + i0,
 						    (void *const *)d_op + i0, d_os + i0, d_on + i0, i1 - i0);
@@ -1009,115 +1026,72 @@ extern "C" int libdeflate_b200_compress_batch_host(struct libdeflate_b200_ctx *c
 						    size_t *h_out_nbytes, size_t n)
 {
 	if (n == 0) return 0;
-	cudaSetDevice(ctx->device);
-	stream_quiesce quiesce(ctx);
-	size_t pb = param_block_bytes(n);
-	size_t res_off = 2 * pb;
-	size_t res_bytes = align_up(n * sizeof(size_t), 256);
-	int rc = ldb_reserve_dev(ctx->d_params, res_off + res_bytes);
+	const host_batch_dir dir = {align_up(n * sizeof(size_t), 256), 1024, false};
+	host_scratch res_own(dir.res_bytes);
+	const size_t *r_on = (const size_t *)res_own.p;
+	if (!r_on) return ldb_fail(cudaErrorMemoryAllocation, "malloc", __FILE__, __LINE__);
+	int rc = host_batch(
+		ctx, dir, h_in, h_in_nbytes, h_out, h_out_avail, n, false, (u8 *)res_own.p,
+		[&](const staged_batch &in, const staged_batch &out, u8 *d_res, size_t i0, size_t i1) {
+			return libdeflate_b200_compress_batch(ctx, format, level, (const void *const *)in.d_ptrs + i0, in.d_sizes + i0,
+							      (void *const *)out.d_ptrs + i0, out.d_sizes + i0, (size_t *)d_res + i0, i1 - i0);
+		},
+		[&](size_t i) { return r_on[i]; });
 	if (rc) return rc;
-	host_scratch hparam_own(res_off + res_bytes);
-	u8 *hparam = (u8 *)hparam_own.p;
-	if (!hparam) return ldb_fail(cudaErrorMemoryAllocation, "malloc", __FILE__, __LINE__);
-	u8 *dparam = (u8 *)ctx->d_params.p;
-	const bool pipelined = pipeline_eligible(ctx, h_in, h_in_nbytes, (const void *const *)h_out, h_out_avail, n);
-	staged_batch in_sb{}, out_sb{};
-	rc = stage_layout(ctx, ctx->d_stage_in, h_in, h_in_nbytes, n, !pipelined, false, dparam, hparam, &in_sb);
-	if (!rc) rc = stage_layout(ctx, ctx->d_stage_out, (const void *const *)h_out, h_out_avail, n, false, true, dparam + pb, hparam + pb, &out_sb);
-	if (!rc) rc = cudaMemcpyAsync(dparam, hparam, 2 * pb, cudaMemcpyHostToDevice, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "H2D params", __FILE__, __LINE__);
-	size_t *d_on = (size_t *)(dparam + res_off);
-	bool out_copied = false;
-	if (!rc && pipelined) {
-		host_span isp = span_of(h_in, h_in_nbytes, n, false), osp = span_of((const void *const *)h_out, h_out_avail, n, true);
-		const size_t imis = (uintptr_t)isp.lo & 15, omis = (uintptr_t)osp.lo & 15;
-		const size_t S = pipe_stages(n, (size_t)(isp.hi - isp.lo) + (size_t)(osp.hi - osp.lo), 1024);
-		pipe_events ev;
-		rc = pipe_events_create(&ev, (int)S);
-		for (size_t k = 0; k < S && !rc; k++) {
-			const size_t i0 = n * k / S, i1 = n * (k + 1) / S;
-			const u8 *ilo = (const u8 *)h_in[i0], *ihi = (const u8 *)h_in[i1 - 1] + h_in_nbytes[i1 - 1];
-			u8 *olo = (u8 *)h_out[i0], *ohi = (u8 *)h_out[i1 - 1] + h_out_avail[i1 - 1];
-			if (ihi > ilo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(in_sb.d_base + imis + (ilo - isp.lo), ilo, (size_t)(ihi - ilo), cudaMemcpyHostToDevice, ctx->stream_h2d));
-			LDB_CUDA_CHECK_RET(cudaEventRecord(ev.in[k], ctx->stream_h2d));
-			LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream, ev.in[k], 0));
-			rc = libdeflate_b200_compress_batch(ctx, format, level, (const void *const *)in_sb.d_ptrs + i0, in_sb.d_sizes + i0,
-							    (void *const *)out_sb.d_ptrs + i0, out_sb.d_sizes + i0, d_on + i0, i1 - i0);
-			if (rc) break;
-			LDB_CUDA_CHECK_RET(cudaEventRecord(ev.done[k], ctx->stream));
-			LDB_CUDA_CHECK_RET(cudaStreamWaitEvent(ctx->stream_d2h, ev.done[k], 0));
-			if (ohi > olo) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(olo, out_sb.d_base + omis + (olo - osp.lo), (size_t)(ohi - olo), cudaMemcpyDeviceToHost, ctx->stream_d2h));
-		}
-		if (!rc) rc = cudaStreamSynchronize(ctx->stream_d2h) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync d2h", __FILE__, __LINE__);
-		pipe_events_destroy(&ev);
-		out_copied = true;
-	} else if (!rc) {
-		rc = libdeflate_b200_compress_batch(ctx, format, level, (const void *const *)in_sb.d_ptrs, in_sb.d_sizes,
-						    (void *const *)out_sb.d_ptrs, out_sb.d_sizes, d_on, n);
-	}
-	size_t *r_on = (size_t *)(hparam + res_off);
-	if (!rc) rc = cudaMemcpyAsync(r_on, d_on, n * sizeof(size_t), cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "D2H sizes", __FILE__, __LINE__);
-	if (!rc) rc = cudaStreamSynchronize(ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-	if (!rc) {
-		if (out_copied) {
-			// done by the pipeline
-		} else if (out_sb.compact) {
-			host_span sp = span_of((const void *const *)h_out, h_out_avail, n, true);
-			size_t mis = (uintptr_t)sp.lo & 15;
-			if (sp.lo)
-				rc = cudaMemcpyAsync((void *)sp.lo, out_sb.d_base + mis, (size_t)(sp.hi - sp.lo), cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "D2H out", __FILE__, __LINE__);
-		} else {
-			rc = ldb_reserve_pinned(ctx->h_pinned, out_sb.slab_bytes);
-			if (!rc) rc = cudaMemcpyAsync(ctx->h_pinned.p, out_sb.d_base, out_sb.slab_bytes - 64, cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "D2H out", __FILE__, __LINE__);
-			if (!rc) rc = cudaStreamSynchronize(ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-			if (!rc)
-				for (size_t i = 0; i < n; i++)
-					if (r_on[i] && h_out[i]) memcpy(h_out[i], (u8 *)ctx->h_pinned.p + out_sb.offsets[i], r_on[i]);
-		}
-		if (!rc) rc = cudaStreamSynchronize(ctx->stream) == cudaSuccess ? 0 : ldb_fail(cudaGetLastError(), "sync", __FILE__, __LINE__);
-		for (size_t i = 0; i < n; i++) h_out_nbytes[i] = r_on[i];
-	}
-	return rc;
+	memcpy(h_out_nbytes, r_on, n * sizeof(size_t));
+	return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// one host buffer <-> the device, for the *_large_host calls
+// ---------------------------------------------------------------------------------
+// Copies nbytes of h into 'stage' at h's 16-byte alignment phase (the device sees the caller's alignment);
+// *d is where its first byte goes.  copy = false only reserves the room.
+static int stage_one(libdeflate_b200_ctx *ctx, ldb_buf &stage, const void *h, size_t nbytes, bool copy, u8 **d)
+{
+	int rc = ldb_reserve_dev(stage, nbytes + 64);
+	if (rc) return rc;
+	*d = (u8 *)stage.p + ((uintptr_t)h & 15);
+	if (copy && nbytes) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(*d, h, nbytes, cudaMemcpyHostToDevice, ctx->stream));
+	return 0;
+}
+
+// nbytes of device memory into h, waited for
+static int read_back(libdeflate_b200_ctx *ctx, void *h, const void *d, size_t nbytes)
+{
+	if (nbytes) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(h, d, nbytes, cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	return 0;
 }
 
 // ---------------------------------------------------------------------------------
 // one large buffer -> one stream (large_kernels.cu)
 // ---------------------------------------------------------------------------------
-// Input bytes per wave (default 1 GiB; LIBDEFLATE_B200_LARGE_WAVE_KB overrides): the context keeps the
-// compressed slots of one wave, not of the whole input.  The stream does not depend on it.
-static size_t ldb_large_wave_pieces(void)
-{
-	size_t kb = (size_t)1 << 20;
-	if (const char *e = getenv("LIBDEFLATE_B200_LARGE_WAVE_KB")) {
-		long v = atol(e);
-		if (v > 0) kb = (size_t)v;
-	}
-	const size_t w = (kb << 10) / LDB_LARGE_PIECE;
-	return w ? w : 1;
-}
-
 extern "C" size_t libdeflate_b200_compress_large_bound(int format, size_t in_nbytes)
 {
-	const size_t wrap = format == LDB_FMT_GZIP ? 18 : (format == LDB_FMT_ZLIB ? 6 : 0);
-	if (in_nbytes <= LDB_LARGE_PIECE) return wrap + ldb_raw_bound(in_nbytes);
+	if (in_nbytes <= LDB_LARGE_PIECE) return wrap_bytes(format) + ldb_raw_bound(in_nbytes);
 	// every piece fits its raw bound; all but the last add their closing empty stored block
 	const size_t full = (in_nbytes - 1) / LDB_LARGE_PIECE;
-	return wrap + full * (ldb_raw_bound(LDB_LARGE_PIECE) + 5) + ldb_raw_bound(in_nbytes - full * LDB_LARGE_PIECE);
+	return wrap_bytes(format) + full * (ldb_raw_bound(LDB_LARGE_PIECE) + 5) + ldb_raw_bound(in_nbytes - full * LDB_LARGE_PIECE);
 }
 
 extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, int format, int level,
 					       const void *d_in, size_t in_nbytes,
 					       void *d_out, size_t out_avail, size_t *d_out_nbytes)
 {
-	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
-	if (level == -1) level = 6;
-	if (level < 0 || level > 12) return ldb_fail(cudaErrorInvalidValue, "level", __FILE__, __LINE__);
+	int rc = check_format(format);
+	if (!rc) rc = check_level(&level);
+	if (rc) return rc;
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
 	const size_t npieces = in_nbytes ? (in_nbytes + LDB_LARGE_PIECE - 1) / LDB_LARGE_PIECE : 1;
-	const size_t wave = npieces < ldb_large_wave_pieces() ? npieces : ldb_large_wave_pieces();
+	// Input bytes per wave (default 1 GiB; LIBDEFLATE_B200_LARGE_WAVE_KB overrides): the context keeps the
+	// compressed slots of one wave, not of the whole input.  The stream does not depend on it.
+	const size_t wave_pieces = std::max((ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_KB", (size_t)1 << 20) << 10) / LDB_LARGE_PIECE, (size_t)1);
+	const size_t wave = npieces < wave_pieces ? npieces : wave_pieces;
 	// ctx->large: in_ptrs | in_nbytes | out_ptrs | out_avail | out_nbytes | offsets | piece | sums | state | slots
 	const size_t a8 = align_up(wave * 8, 256), a4 = align_up(wave * 4, 256);
 	const size_t slots_off = 6 * a8 + 2 * a4 + 256;
-	int rc = ldb_reserve_dev(ctx->large, slots_off + (npieces > 1 ? wave * LDB_LARGE_SLOT : 0));
+	rc = ldb_reserve_dev(ctx->large, slots_off + (npieces > 1 ? wave * LDB_LARGE_SLOT : 0));
 	if (rc) return rc;
 	u8 *b = (u8 *)ctx->large.p;
 	ldb_large_args g;
@@ -1168,10 +1142,7 @@ extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, i
 		a.n = g.count;
 		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_setup(g, ctx->stream); });
 		if (rc) return rc;
-		if (format == LDB_FMT_GZIP)
-			rc = ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, a.in_ptrs, a.in_nbytes, nullptr, g.sums, g.count, ctx->cfg, ctx->stream); });
-		else if (format == LDB_FMT_ZLIB)
-			rc = ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32(a.in_ptrs, a.in_nbytes, nullptr, g.sums, g.count, ctx->cfg, ctx->stream); });
+		rc = launch_checksum(ctx, format, a.in_ptrs, a.in_nbytes, g.sums, g.count);
 		if (rc) return rc;
 		rc = ldb_timed_launch(ctx, LDB_K_DEFLATE, [&] { return ldb_launch_deflate(a, ctx->cfg, ctx->stream); });
 		if (rc) return rc;
@@ -1189,21 +1160,18 @@ extern "C" int libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *c
 	*out_nbytes = 0;
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
 	stream_quiesce quiesce(ctx);
-	int rc = ldb_reserve_dev(ctx->d_stage_in, in_nbytes + 64);
+	u8 *d_in;
+	int rc = stage_one(ctx, ctx->d_stage_in, in, in_nbytes, true, &d_in);
 	if (!rc) rc = ldb_reserve_dev(ctx->d_stage_out, out_avail + 64);
 	if (!rc) rc = ldb_reserve_dev(ctx->d_params, 256);
 	if (rc) return rc;
-	// (the input keeps its 16-byte alignment phase on the device)
-	const u8 *d_in = (const u8 *)ctx->d_stage_in.p + ((uintptr_t)in & 15);
 	size_t *d_res = (size_t *)ctx->d_params.p;
-	if (in_nbytes) LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)d_in, in, in_nbytes, cudaMemcpyHostToDevice, ctx->stream));
 	rc = libdeflate_b200_compress_large(ctx, format, level, d_in, in_nbytes, ctx->d_stage_out.p, out_avail, d_res);
 	if (rc) return rc;
 	size_t r = 0;
-	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(&r, d_res, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
-	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
-	if (r) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(out, ctx->d_stage_out.p, r, cudaMemcpyDeviceToHost, ctx->stream));
-	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	rc = read_back(ctx, &r, d_res, sizeof(r));
+	if (!rc) rc = read_back(ctx, out, ctx->d_stage_out.p, r);
+	if (rc) return rc;
 	*out_nbytes = r;
 	return 0;
 }
@@ -1211,20 +1179,6 @@ extern "C" int libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *c
 // ---------------------------------------------------------------------------------
 // one large stream -> its bytes (large_inflate.cu, inflate_kernel.cu segment mode; DESIGN.md 4.6)
 // ---------------------------------------------------------------------------------
-// Minimum distance in input bytes between two split points (LIBDEFLATE_B200_LARGE_SPLIT_MIN overrides;
-// default 16 KiB, below half of what a compress_large piece compresses to), the most segments one
-// wave decodes (LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS; the token budget bounds a wave as well), and how far
-// a speculative segment may read past its next split point before it gives up (LIBDEFLATE_B200_LARGE_OVERRUN,
-// default 4 MiB; real blocks are far shorter).
-static size_t ldb_env_size(const char *name, size_t dflt)
-{
-	if (const char *e = getenv(name)) {
-		long long v = atoll(e);
-		if (v > 0) return (size_t)v;
-	}
-	return dflt;
-}
-
 // host-side bump layout of one device buffer
 struct dev_layout {
 	std::vector<u8> h;
@@ -1327,53 +1281,41 @@ static int li_resolve(libdeflate_b200_ctx *ctx, const ldb_inflate_args &a0, cons
 	return ldb_timed_launch(ctx, LDB_K_RESOLVE, [&] { return ldb_launch_inflate_resolve_lit(a, hilit, ctx->cfg, ctx->stream); });
 }
 
-extern "C" size_t libdeflate_b200_decompress_large_segments(struct libdeflate_b200_ctx *ctx) { return ctx->li_segments; }
-
-extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
-						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
-						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+// Split points of one stream (bit offsets into the input, ascending, at least LIBDEFLATE_B200_LARGE_SPLIT_MIN
+// bytes apart; default 16 KiB, below half of what a compress_large piece compresses to): its sync points, or,
+// when it has none, the block starts the finder lists.  *found: the split points are found block starts.
+static int li_split_points(libdeflate_b200_ctx *ctx, const u8 *in, size_t n, u64 data_end, std::vector<u64> &split, bool *found)
 {
-	if (format < LDB_FMT_RAW || format > LDB_FMT_GZIP) return ldb_fail(cudaErrorInvalidValue, "format", __FILE__, __LINE__);
-	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
-	ctx->li_segments = 0;
-	const u8 *in = (const u8 *)d_in;
-	u8 *out = (u8 *)d_out;
-	const size_t n = in_nbytes;
-	const u32 footer = format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0);
-	const u64 data_end = n >= footer ? n - footer : 0;	// the DEFLATE data ends before the trailer
-	int rc;
-
 	// ---- 1. sync points: every 00 00 FF FF, then split points at least split_min apart ----------------
 	// (split points and segment starts are bit offsets into the input; a sync point's is 8 x its byte)
-	std::vector<u64> split, c8;
-	{
-		const size_t tiles = ldb_sync_scan_tiles(n);
-		if (tiles) {
-			rc = ldb_reserve_dev(ctx->li_scan, tiles * 12 + 512);
+	std::vector<u64> c8;
+	int rc;
+	const size_t tiles = ldb_sync_scan_tiles(n);
+	if (tiles) {
+		rc = ldb_reserve_dev(ctx->li_scan, tiles * 12 + 512);
+		if (rc) return rc;
+		u32 *d_counts = (u32 *)ctx->li_scan.p;
+		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_sync_scan_count(in, n, d_counts, tiles, ctx->stream); });
+		if (rc) return rc;
+		std::vector<u32> counts(tiles);
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(counts.data(), d_counts, tiles * 4, cudaMemcpyDeviceToHost, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+		std::vector<u64> toff(tiles);
+		u64 total = 0;
+		for (size_t t = 0; t < tiles; t++) { toff[t] = total; total += counts[t]; }
+		if (total) {
+			const size_t o_off = align_up(tiles * 4, 256);
+			const size_t o_cand = o_off + align_up(tiles * 8, 256);
+			rc = ldb_reserve_dev(ctx->li_scan, o_cand + total * 8);
 			if (rc) return rc;
-			u32 *d_counts = (u32 *)ctx->li_scan.p;
-			rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_sync_scan_count(in, n, d_counts, tiles, ctx->stream); });
+			u8 *b = (u8 *)ctx->li_scan.p;
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(b + o_off, toff.data(), tiles * 8, cudaMemcpyHostToDevice, ctx->stream));
+			rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_sync_scan_write(in, n, (const u64 *)(b + o_off), (u64 *)(b + o_cand), tiles, ctx->stream); });
 			if (rc) return rc;
-			std::vector<u32> counts(tiles);
-			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(counts.data(), d_counts, tiles * 4, cudaMemcpyDeviceToHost, ctx->stream));
+			std::vector<u64> cand(total);
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(cand.data(), b + o_cand, total * 8, cudaMemcpyDeviceToHost, ctx->stream));
 			LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
-			std::vector<u64> toff(tiles);
-			u64 total = 0;
-			for (size_t t = 0; t < tiles; t++) { toff[t] = total; total += counts[t]; }
-			if (total) {
-				const size_t o_off = align_up(tiles * 4, 256);
-				const size_t o_cand = o_off + align_up(tiles * 8, 256);
-				rc = ldb_reserve_dev(ctx->li_scan, o_cand + total * 8);
-				if (rc) return rc;
-				u8 *b = (u8 *)ctx->li_scan.p;
-				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(b + o_off, toff.data(), tiles * 8, cudaMemcpyHostToDevice, ctx->stream));
-				rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_sync_scan_write(in, n, (const u64 *)(b + o_off), (u64 *)(b + o_cand), tiles, ctx->stream); });
-				if (rc) return rc;
-				std::vector<u64> cand(total);
-				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(cand.data(), b + o_cand, total * 8, cudaMemcpyDeviceToHost, ctx->stream));
-				LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
-				for (u64 c : cand) c8.push_back(8 * c);
-			}
+			for (u64 c : cand) c8.push_back(8 * c);
 		}
 	}
 	const u64 dmin = 8 * ldb_env_size("LIBDEFLATE_B200_LARGE_SPLIT_MIN", 16384);
@@ -1386,9 +1328,9 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	// ---- 1b. no sync split point: candidate block starts at bit offsets of the DEFLATE data ------------
 	// (not below 4 split spacings of data: two or three segments would not repay the finder, the symbol
 	// planes and the window chain)
-	bool found = false;	// split points are found block starts, not sync points
+	*found = false;
 	if (split.empty() && 8 * (u64)data_end >= 4 * dmin) {
-		found = true;
+		*found = true;
 		c8.clear();
 		const u64 cap0 = data_end / 512 + 1024;		// real blocks are tens of KiB apart; a second run takes more
 		for (u64 cap = cap0;;) {
@@ -1412,6 +1354,30 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		c8.erase(std::unique(c8.begin(), c8.end()), c8.end());
 		thin();
 	}
+	return 0;
+}
+
+extern "C" size_t libdeflate_b200_decompress_large_segments(struct libdeflate_b200_ctx *ctx) { return ctx->li_segments; }
+
+extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
+						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+{
+	int rc = check_format(format);
+	if (rc) return rc;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	ctx->li_segments = 0;
+	const u8 *in = (const u8 *)d_in;
+	u8 *out = (u8 *)d_out;
+	const size_t n = in_nbytes;
+	const u32 footer = format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0);
+	const u64 data_end = n >= footer ? n - footer : 0;	// the DEFLATE data ends before the trailer
+
+	// ---- 1. split points: sync points, else found block starts -----------------------------------------
+	std::vector<u64> split;
+	bool found;	// split points are found block starts, not sync points
+	rc = li_split_points(ctx, in, n, data_end, split, &found);
+	if (rc) return rc;
 	const size_t nseg = split.size() + 1;
 	// the split list lives at the start of li_scan for the whole call
 	if (!split.empty()) {
@@ -1442,9 +1408,12 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	std::vector<chain_rec> chain;
 	ldb_large_verdict v = {};
 	v.result = -1;
-	const u64 budget = ldb_token_budget();
+	const u64 budget = token_budget_bytes();
+	// the most segments one wave decodes (the token budget bounds a wave as well)
 	const size_t wave_max = ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS", (size_t)1 << 20);
-	// (found block starts only: a stream split at sync points keeps the uncapped decode it always had)
+	// how far a speculative segment may read past its next split point before it gives up (default 4 MiB; real
+	// blocks are far shorter).  Found block starts only: a stream split at sync points keeps the uncapped decode
+	// it always had.
 	const u64 overrun = found ? 8 * (u64)ldb_env_size("LIBDEFLATE_B200_LARGE_OVERRUN", (size_t)4 << 20) : 0;
 	u64 G = 0;
 	size_t cur = 0;		// the next chain segment
@@ -1655,10 +1624,7 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		for (size_t i = 0; i < nch; i++) { hp[i] = out + chain[i].G; hl[i] = chain[i].len; }
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)d_ptrs, hp.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_lens, hl.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
-		if (format == LDB_FMT_GZIP)
-			rc = ldb_timed_launch(ctx, LDB_K_CRC32, [&] { return ldb_launch_crc32(ctx->d_crc_tables, d_ptrs, d_lens, nullptr, d_sums, nch, ctx->cfg, ctx->stream); });
-		else
-			rc = ldb_timed_launch(ctx, LDB_K_ADLER32, [&] { return ldb_launch_adler32(d_ptrs, d_lens, nullptr, d_sums, nch, ctx->cfg, ctx->stream); });
+		rc = launch_checksum(ctx, format, d_ptrs, d_lens, d_sums, nch);
 		if (rc) return rc;
 	}
 	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_inflate_finish(d_sums, d_lens, nch, format, v, d_actual_in, d_actual_out, d_result, ctx->stream); });
@@ -1670,25 +1636,23 @@ extern "C" int libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx 
 {
 	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
 	stream_quiesce quiesce(ctx);
-	int rc = ldb_reserve_dev(ctx->d_stage_in, in_nbytes + 64);
-	if (!rc) rc = ldb_reserve_dev(ctx->d_stage_out, out_avail + 64);
+	// (both sides keep their 16-byte alignment phase on the device)
+	u8 *d_in, *d_out;
+	int rc = stage_one(ctx, ctx->d_stage_in, in, in_nbytes, true, &d_in);
+	if (!rc) rc = stage_one(ctx, ctx->d_stage_out, out, out_avail, false, &d_out);
 	if (!rc) rc = ldb_reserve_dev(ctx->d_params, 256);
 	if (rc) return rc;
-	// (both sides keep their 16-byte alignment phase on the device)
-	u8 *d_in = (u8 *)ctx->d_stage_in.p + ((uintptr_t)in & 15);
-	u8 *d_out = (u8 *)ctx->d_stage_out.p + ((uintptr_t)out & 15);
 	size_t *d_res = (size_t *)ctx->d_params.p;	// actual_in, actual_out, result
-	if (in_nbytes) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_in, in, in_nbytes, cudaMemcpyHostToDevice, ctx->stream));
 	LDB_CUDA_CHECK_RET(cudaMemsetAsync(d_res, 0, 3 * sizeof(size_t), ctx->stream));
 	rc = libdeflate_b200_decompress_large(ctx, format, flags, d_in, in_nbytes, d_out, out_avail, d_res, d_res + 1, (int32_t *)(d_res + 2));
 	if (rc) return rc;
 	size_t h[3];
-	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(h, d_res, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	rc = read_back(ctx, h, d_res, sizeof(h));
+	if (rc) return rc;
 	const int32_t r = (int32_t)h[2];
-	if (r == LDB_SUCCESS && h[1]) {
-		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(out, d_out, h[1], cudaMemcpyDeviceToHost, ctx->stream));
-		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+	if (r == LDB_SUCCESS) {
+		rc = read_back(ctx, out, d_out, h[1]);
+		if (rc) return rc;
 	}
 	if (result) *result = r;
 	if (actual_in) *actual_in = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[0] : 0;
@@ -1710,14 +1674,12 @@ static void (*g_free)(void *) = free;
 static const u8 LDB_BGZF_EOF[28] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 'B', 'C', 2, 0, 27, 0,
 				    3, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 
-static size_t gzip_bound_of(size_t n) { return 5 * ((n + 4999) / 5000 ? (n + 4999) / 5000 : 1) + n + 18; }
-
 extern "C" size_t libdeflate_b200_bgzf_compress_bound(size_t in_nbytes)
 {
 	const size_t B = LIBDEFLATE_B200_BGZF_BLOCK;
 	const size_t full = in_nbytes / B, tail = in_nbytes % B;
-	size_t total = full * (gzip_bound_of(B) + 8) + sizeof(LDB_BGZF_EOF);
-	if (tail) total += gzip_bound_of(tail) + 8;
+	size_t total = full * (wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(B) + 8) + sizeof(LDB_BGZF_EOF);
+	if (tail) total += wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(tail) + 8;
 	return total;
 }
 
@@ -1726,7 +1688,7 @@ extern "C" int libdeflate_b200_bgzf_compress(struct libdeflate_b200_ctx *ctx, in
 {
 	const size_t B = LIBDEFLATE_B200_BGZF_BLOCK;
 	const size_t nblk = (in_nbytes + B - 1) / B;
-	const size_t slot = (gzip_bound_of(B) + 15) & ~(size_t)15;
+	const size_t slot = (wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(B) + 15) & ~(size_t)15;
 	*out_nbytes = 0;
 	size_t pos = 0;
 	u8 *o = (u8 *)out;
@@ -1914,17 +1876,15 @@ extern "C" void libdeflate_free_decompressor(struct libdeflate_decompressor *d)
 extern "C" size_t libdeflate_deflate_compress_bound(struct libdeflate_compressor *c, size_t in_nbytes)
 {
 	(void)c;
-	size_t max_blocks = (in_nbytes + 4999) / 5000;
-	if (max_blocks < 1) max_blocks = 1;
-	return 5 * max_blocks + in_nbytes;
+	return ldb_raw_bound(in_nbytes);
 }
 extern "C" size_t libdeflate_zlib_compress_bound(struct libdeflate_compressor *c, size_t in_nbytes)
 {
-	return 6 + libdeflate_deflate_compress_bound(c, in_nbytes);
+	return wrap_bytes(LDB_FMT_ZLIB) + libdeflate_deflate_compress_bound(c, in_nbytes);
 }
 extern "C" size_t libdeflate_gzip_compress_bound(struct libdeflate_compressor *c, size_t in_nbytes)
 {
-	return 18 + libdeflate_deflate_compress_bound(c, in_nbytes);
+	return wrap_bytes(LDB_FMT_GZIP) + libdeflate_deflate_compress_bound(c, in_nbytes);
 }
 
 static bool is_device_pointer(const void *p)
@@ -1936,6 +1896,38 @@ static bool is_device_pointer(const void *p)
 		return false;
 	}
 	return at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+}
+
+// The one-chunk parameter block of the classic calls' device / mixed-pointer path, uploaded to ctx->d_params
+// (*d): host buffers are staged (the input copied, room reserved for the output), device buffers used in place.
+struct single_params {
+	const void *in;
+	size_t in_n;
+	void *out;
+	size_t out_n;
+	size_t ain, aout;	// results (compress: aout = the stream size)
+	int32_t res;
+};
+static int stage_single(libdeflate_b200_ctx *ctx, const void *in, size_t in_n, bool din, void *out, size_t out_n, bool dout,
+			single_params *p, single_params **d)
+{
+	*p = {in, in_n, out, out_n, 0, 0, 1};
+	int rc = ldb_reserve_dev(ctx->d_params, 4096);
+	if (rc) return rc;
+	if (!din) {
+		rc = ldb_reserve_dev(ctx->d_stage_in, in_n + 64);
+		if (rc) return rc;
+		if (in_n) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->d_stage_in.p, in, in_n, cudaMemcpyHostToDevice, ctx->stream));
+		p->in = ctx->d_stage_in.p;
+	}
+	if (!dout) {
+		rc = ldb_reserve_dev(ctx->d_stage_out, out_n + 64);
+		if (rc) return rc;
+		p->out = ctx->d_stage_out.p;
+	}
+	*d = (single_params *)ctx->d_params.p;
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(*d, p, sizeof(*p), cudaMemcpyHostToDevice, ctx->stream));
+	return 0;
 }
 
 static size_t single_compress(struct libdeflate_compressor *c, int format, const void *in, size_t in_nbytes,
@@ -1957,33 +1949,11 @@ static size_t single_compress(struct libdeflate_compressor *c, int format, const
 		rc = libdeflate_b200_compress_batch_host(ctx, format, c->level, hin, &in_nbytes, hout, &out_avail, &r, 1);
 	} else {
 		// mixed / device buffers: stage only what is on the host
-		rc = ldb_reserve_dev(ctx->d_params, 4096);
-		u8 *dp = (u8 *)ctx->d_params.p;
-		const void *d_in = hin[0];
-		void *d_out = out;
-		if (!rc && !din) {
-			rc = ldb_reserve_dev(ctx->d_stage_in, in_nbytes + 64);
-			if (!rc && in_nbytes) rc = libdeflate_b200_memcpy_h2d(ctx, ctx->d_stage_in.p, hin[0], in_nbytes);
-			d_in = ctx->d_stage_in.p;
-		}
-		if (!rc && !dout) {
-			rc = ldb_reserve_dev(ctx->d_stage_out, out_avail + 64);
-			d_out = ctx->d_stage_out.p;
-		}
-		struct { const void *in; size_t in_n; void *out; size_t out_n; size_t res; } hp = {d_in, in_nbytes, d_out, out_avail, 0};
-		if (!rc) rc = libdeflate_b200_memcpy_h2d(ctx, dp, &hp, sizeof(hp));
-		if (!rc)
-			rc = libdeflate_b200_compress_batch(ctx, format, c->level, (const void *const *)(dp + offsetof(decltype(hp), in)),
-							    (const size_t *)(dp + offsetof(decltype(hp), in_n)),
-							    (void *const *)(dp + offsetof(decltype(hp), out)),
-							    (const size_t *)(dp + offsetof(decltype(hp), out_n)),
-							    (size_t *)(dp + offsetof(decltype(hp), res)), 1);
-		if (!rc) rc = libdeflate_b200_memcpy_d2h(ctx, &r, dp + offsetof(decltype(hp), res), sizeof(size_t));
-		if (!rc) rc = libdeflate_b200_ctx_sync(ctx);
-		if (!rc && !dout && r) {
-			rc = libdeflate_b200_memcpy_d2h(ctx, out, d_out, r);
-			if (!rc) rc = libdeflate_b200_ctx_sync(ctx);
-		}
+		single_params p, *d;
+		rc = stage_single(ctx, hin[0], in_nbytes, din, out, out_avail, dout, &p, &d);
+		if (!rc) rc = libdeflate_b200_compress_batch(ctx, format, c->level, &d->in, &d->in_n, &d->out, &d->out_n, &d->aout, 1);
+		if (!rc) rc = read_back(ctx, &r, &d->aout, sizeof(r));
+		if (!rc && !dout) rc = read_back(ctx, out, p.out, r);
 	}
 	if (rc) ldb_die("libdeflate_*_compress");
 	return r;
@@ -2023,35 +1993,14 @@ static enum libdeflate_result single_decompress(struct libdeflate_decompressor *
 	if (!din && !dout) {
 		rc = libdeflate_b200_decompress_batch_host(ctx, format, flags, hin, &in_nbytes, hout, &out_avail, &ain, &aout, &res, 1);
 	} else {
-		rc = ldb_reserve_dev(ctx->d_params, 4096);
-		u8 *dp = (u8 *)ctx->d_params.p;
-		const void *d_in = hin[0];
-		void *d_out = hout[0];
-		if (!rc && !din) {
-			rc = ldb_reserve_dev(ctx->d_stage_in, in_nbytes + 64);
-			if (!rc && in_nbytes) rc = libdeflate_b200_memcpy_h2d(ctx, ctx->d_stage_in.p, hin[0], in_nbytes);
-			d_in = ctx->d_stage_in.p;
-		}
-		if (!rc && !dout) {
-			rc = ldb_reserve_dev(ctx->d_stage_out, out_avail + 64);
-			d_out = ctx->d_stage_out.p;
-		}
-		struct P { const void *in; size_t in_n; void *out; size_t out_n; size_t ain; size_t aout; int32_t res; } hp = {d_in, in_nbytes, d_out, out_avail, 0, 0, 1};
-		if (!rc) rc = libdeflate_b200_memcpy_h2d(ctx, dp, &hp, sizeof(hp));
-		if (!rc)
-			rc = libdeflate_b200_decompress_batch(ctx, format, flags, (const void *const *)(dp + offsetof(P, in)),
-							      (const size_t *)(dp + offsetof(P, in_n)), (void *const *)(dp + offsetof(P, out)),
-							      (const size_t *)(dp + offsetof(P, out_n)), (size_t *)(dp + offsetof(P, ain)),
-							      (size_t *)(dp + offsetof(P, aout)), (int32_t *)(dp + offsetof(P, res)), 1);
-		if (!rc) rc = libdeflate_b200_memcpy_d2h(ctx, &hp, dp, sizeof(hp));
-		if (!rc) rc = libdeflate_b200_ctx_sync(ctx);
-		ain = hp.ain;
-		aout = hp.aout;
-		res = hp.res;
-		if (!rc && !dout && (res == LIBDEFLATE_SUCCESS || res == LIBDEFLATE_SHORT_OUTPUT) && aout) {
-			rc = libdeflate_b200_memcpy_d2h(ctx, hout[0], d_out, aout);
-			if (!rc) rc = libdeflate_b200_ctx_sync(ctx);
-		}
+		single_params p, *d;
+		rc = stage_single(ctx, hin[0], in_nbytes, din, hout[0], out_avail, dout, &p, &d);
+		if (!rc) rc = libdeflate_b200_decompress_batch(ctx, format, flags, &d->in, &d->in_n, &d->out, &d->out_n, &d->ain, &d->aout, &d->res, 1);
+		if (!rc) rc = read_back(ctx, &p, d, sizeof(p));
+		ain = p.ain;
+		aout = p.aout;
+		res = p.res;
+		if (!rc && !dout && (res == LIBDEFLATE_SUCCESS || res == LIBDEFLATE_SHORT_OUTPUT)) rc = read_back(ctx, hout[0], p.out, aout);
 	}
 	if (rc) ldb_die("libdeflate_*_decompress");
 	if (res == LIBDEFLATE_SUCCESS) {
@@ -2123,9 +2072,11 @@ static uint32_t single_checksum(bool is_crc, uint32_t init, const void *buffer, 
 	if (!rc) rc = libdeflate_b200_memcpy_d2h(ctx, vals, dp + off_vals, nseg * sizeof(u32));
 	if (!rc) rc = libdeflate_b200_ctx_sync(ctx);
 	if (rc) ldb_die(is_crc ? "libdeflate_crc32" : "libdeflate_adler32");
+	u32 xp[64];	// x^(8 * 2^i) mod G, for the CRC-32 combine
+	xp[0] = 0x00800000u;
+	for (int i = 1; i < 64; i++) xp[i] = ldb_mulmodp(xp[i - 1], xp[i - 1]);
 	u32 v = vals[0];
-	for (size_t i = 1; i < nseg; i++)
-		v = is_crc ? h_crc32_combine(v, vals[i], sizes[i]) : h_adler32_combine(v, vals[i], sizes[i]);
+	for (size_t i = 1; i < nseg; i++) v = ldb_sum_combine(is_crc ? LDB_FMT_GZIP : LDB_FMT_ZLIB, xp, v, vals[i], sizes[i]);
 	free(hp);
 	return v;
 }
