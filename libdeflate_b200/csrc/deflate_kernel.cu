@@ -10,6 +10,8 @@
 // (level 0 and inputs <= 55 - 4*level bytes: ref deflate_compress_none,
 // lib/deflate_compress.c:2393-2443).  The LZ77 + Huffman path is in
 // deflate_lz_kernel.cuh.
+#include <stdlib.h>
+
 #include "ldb_common.cuh"
 
 #define DEF_THREADS 256
@@ -57,7 +59,17 @@ ldb_deflate_stored_kernel(ldb_deflate_args a)
 
 #include "deflate_lz_kernel.cuh"
 
-int ldb_deflate_grid(const ldb_launch_cfg &cfg) { return cfg.num_sms; }
+// One CTA per SM.  LIBDEFLATE_B200_DEFLATE_CTAS=k caps the grid at k CTAs (tests: every CTA then
+// compresses many chunks in a row, which is where a chunk's last step and the next one's step 0 meet).
+int ldb_deflate_grid(const ldb_launch_cfg &cfg)
+{
+	int g = cfg.num_sms;
+	if (const char *e = getenv("LIBDEFLATE_B200_DEFLATE_CTAS")) {
+		const int k = atoi(e);
+		if (k > 0 && k < g) g = k;
+	}
+	return g;
+}
 
 int ldb_launch_deflate(const ldb_deflate_args &a, const ldb_launch_cfg &cfg, void *stream)
 {

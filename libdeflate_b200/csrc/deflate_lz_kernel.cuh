@@ -73,6 +73,8 @@
 #define LZ_PWARPS    12
 #endif
 #define LZ_BAR_P     1				// named barrier of the parse/flush group
+#define LZ_BAR_S     2				// named barrier of the search group (a chunk's step 0 beside the last step of the one before)
+#define LZ_BAR_H     3				// hand-over: the search group arrives when that step 0 has inserted pass 0
 #ifndef LZ_PF
 #define LZ_PF        4				// parse: windows of per-position results in flight per warp
 #endif
@@ -137,6 +139,8 @@ struct lz_vars {
 	u32 dict, nonfinal;	// the chunk's ldb_deflate_args::piece fields
 	u32 spec_last;		// parse: last round in which a window's entry changed
 	u32 spec_first;		// parse: first window the last allowed round changed
+	u32 prefetched;		// chunk: 1 = fetched during the previous chunk, 2 = and its step 0 ran beside that chunk's last step
+	u32 nx_min_len, nx_far4;	// min_len / far4_dist of a chunk whose step 0 runs beside the previous chunk's last step
 };
 static_assert(sizeof(lz_vars) <= 256, "lz_vars fits its shared-memory slot");
 
@@ -202,17 +206,18 @@ __device__ __forceinline__ u32 lz_ld32(const u8 *ring, u32 pos)
 __device__ __forceinline__ u32 lz_ld8(const u8 *ring, u32 pos) { return ring[pos & (LZ_RING - 1)]; }
 __device__ __forceinline__ u32 lz_hash(u32 v) { return (v * 0x1E35A7BDu) >> (32 - LZ_HASH_BITS); }	// ref: matchfinder_common.h:168-172
 
-// ---- TMA bulk load of one segment into the ring -------------------------------------
-__device__ __forceinline__ void lz_load_segment(u8 *sm, lz_vars *v, const u8 *in, u32 from, u32 to)
+// ---- TMA bulk load of one segment into the ring, by a group of gn threads (gt: rank in it, bar: its barrier)
+template <typename Bar>
+__device__ __forceinline__ void lz_load_segment(u8 *sm, lz_vars *v, const u8 *in, u32 from, u32 to, u32 gt, u32 gn, Bar bar)
 {
 	u8 *ring = sm + LZ_SM_RING;
 	u32 len = to - from;
 	u32 bulk = (((uintptr_t)(in + from) & 15) == 0) ? (len & ~15u) : 0;
-	__syncthreads();	// every earlier generic-proxy access to the slots being overwritten is done
+	bar();	// every earlier generic-proxy access to the slots being overwritten is done
 #ifndef LDB_EMU
 	if (bulk) {
 		u32 mbar = (u32)__cvta_generic_to_shared(&v->mbar);
-		if (threadIdx.x == 0) {
+		if (gt == 0) {
 			u32 dst = (u32)__cvta_generic_to_shared(ring + (from & (LZ_RING - 1)));
 			asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 			asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(bulk) : "memory");
@@ -227,12 +232,12 @@ __device__ __forceinline__ void lz_load_segment(u8 *sm, lz_vars *v, const u8 *in
 		}
 	}
 #else
-	for (u32 i = threadIdx.x; i < bulk; i += LZ_THREADS) ring[(from + i) & (LZ_RING - 1)] = in[from + i];
+	for (u32 i = gt; i < bulk; i += gn) ring[(from + i) & (LZ_RING - 1)] = in[from + i];
 #endif
-	for (u32 i = bulk + threadIdx.x; i < len; i += LZ_THREADS) ring[(from + i) & (LZ_RING - 1)] = in[from + i];
-	__syncthreads();
-	if (bulk && threadIdx.x == 0) v->tma_phase ^= 1;
-	__syncthreads();
+	for (u32 i = bulk + gt; i < len; i += gn) ring[(from + i) & (LZ_RING - 1)] = in[from + i];
+	bar();
+	if (bulk && gt == 0) v->tma_phase ^= 1;
+	bar();
 }
 
 // ---- length / offset slot helpers (Appendix A; ref: deflate_compress.c:237-308) ------
@@ -345,11 +350,17 @@ __device__ __forceinline__ void lz_gen_codes_serial(const u8 *lens, u32 nsyms, u
 // tuning builds only: cycles per phase, summed over all CTAs, clocked separately by thread 0 (first
 // warp of the parse/flush group) and by the first thread of the search group; whole-CTA phases appear
 // in both.  (The compiler may read the clock before a barrier wait, so a phase in which the clocking
-// thread finishes early is under-counted and the wait shows up in the next one.)
-__device__ unsigned long long ldb_lz_timing[2][16];
+// thread finishes early is under-counted and the wait shows up in the next one.)  Slots 16 and 17 clock
+// whole stretches that the phases 0-14 already cover: a chunk's last step (from its start to its join)
+// and step 0's load and insertion.
+__device__ unsigned long long ldb_lz_timing[2][18];
 #define LZ_T(k) do { if (tid == 0 || tid == 32 * LZ_PWARPS) { long long t_ = clock64(); tacc[k] += t_ - tlast; tlast = t_; } } while (0)
+#define LZ_TSPAN_BEGIN() do { if (tid == 0 || tid == 32 * LZ_PWARPS) tspan = clock64(); } while (0)
+#define LZ_TSPAN_END(k) do { if (tid == 0 || tid == 32 * LZ_PWARPS) tacc[k] += clock64() - tspan; } while (0)
 #else
 #define LZ_T(k) do { } while (0)
+#define LZ_TSPAN_BEGIN() do { } while (0)
+#define LZ_TSPAN_END(k) do { } while (0)
 #endif
 
 #ifdef LZ_SPEC_STATS
@@ -396,33 +407,36 @@ __device__ __forceinline__ u32 lz_same_key_mask(u32 key, bool valid)
 //      the same-slice lane mask): every list ends up sorted by position;
 //  (4) warp s links list s, 32 entries at a time: predecessors inside the batch come from
 //      the same-hash lane mask, the others from head[].  Same links as a serial insertion.
+// Run by a group of gw warps (warp: rank in the group, tid: thread rank, bar: its barrier); with fewer
+// warps than slices a warp links several lists in turn, which gives the same links.
+template <typename Bar>
 __device__ __forceinline__ void lz_insert_pass_par(const u8 *ring, u16 *head, u16 *nextt, u32 *cmat,
-						   u32 b0, u32 pend, u32 n, u32 tid, u32 lane, u32 warp
+						   u32 b0, u32 pend, u32 n, u32 tid, u32 lane, u32 warp, u32 gw, Bar bar
 #ifdef LZ_TIMING
 						   , long long *tacc, long long &tlast
 #endif
 						   )
 {
-	static_assert(LZ_WARPS >= LZ_NSL && (LZ_WARPS * LZ_NSL + 2 * LZ_NSL) * 4 <= 8192, "one linking warp per slice");
+	static_assert((LZ_WARPS * LZ_NSL + 2 * LZ_NSL) * 4 <= 8192, "count matrix fits the start of region R");
 	u32 *sbase = cmat + LZ_WARPS * LZ_NSL, *stot = sbase + LZ_NSL;
 	const u32 lt = (1u << lane) - 1;
 	const u32 LB = (b0 + LZ_PASS) & 0xffff;
-	const u32 ntiles = (pend - b0 + 31) >> 5, tpw = (ntiles + LZ_WARPS - 1) / LZ_WARPS;
+	const u32 ntiles = (pend - b0 + 31) >> 5, tpw = (ntiles + gw - 1) / gw;
 	const u32 r0 = b0 + warp * tpw * 32;
 	const u32 r1 = r0 + tpw * 32 < pend ? r0 + tpw * 32 : pend;
-	for (u32 i = tid; i < LZ_WARPS * LZ_NSL + 2 * LZ_NSL; i += LZ_THREADS) cmat[i] = 0;
-	__syncthreads();
+	for (u32 i = tid; i < LZ_WARPS * LZ_NSL + 2 * LZ_NSL; i += 32 * gw) cmat[i] = 0;
+	bar();
 	for (u32 p = r0 + lane; p < r1; p += 32) {
 		const u32 hv = p + 4 <= n ? lz_hash(lz_ld32(ring, p)) : 0xffffu;
 		nextt[p & 0xffff] = (u16)hv;
 		if (hv != 0xffffu) atomicAdd(&cmat[warp * LZ_NSL + (hv >> (LZ_HASH_BITS - LZ_NSL_BITS))], 1u);
 	}
-	__syncthreads();
+	bar();
 	LZ_T(12);	// insertion: hashing
 	if (warp == 0) {
 		u32 run = 0;
 		if (lane < LZ_NSL)
-			for (u32 w = 0; w < LZ_WARPS; w++) {
+			for (u32 w = 0; w < gw; w++) {
 				const u32 c = cmat[w * LZ_NSL + lane];
 				cmat[w * LZ_NSL + lane] = run;
 				run += c;
@@ -434,7 +448,7 @@ __device__ __forceinline__ void lz_insert_pass_par(const u8 *ring, u16 *head, u1
 		}
 		if (lane < LZ_NSL) { sbase[lane] = incl - run; stot[lane] = run; }
 	}
-	__syncthreads();
+	bar();
 	for (u32 t = 0; t < tpw; t++) {
 		const u32 p = r0 + 32 * t + lane;
 		const u32 hv = p < r1 ? nextt[p & 0xffff] : 0xffffu;
@@ -449,11 +463,11 @@ __device__ __forceinline__ void lz_insert_pass_par(const u8 *ring, u16 *head, u1
 		}
 		__syncwarp();
 	}
-	__syncthreads();
+	bar();
 	LZ_T(13);	// insertion: slice lists
-	if (warp < LZ_NSL) {
-		const u32 cnt = stot[warp];
-		const u16 *mylist = nextt + LB + sbase[warp];
+	for (u32 s = warp; s < LZ_NSL; s += gw) {
+		const u32 cnt = stot[s];
+		const u16 *mylist = nextt + LB + sbase[s];
 		u32 p16n = lane < cnt ? mylist[lane] : 0;
 		u32 hn = lane < cnt ? nextt[p16n] : 0;
 		for (u32 b = 0; b < cnt; b += 32) {
@@ -475,7 +489,7 @@ __device__ __forceinline__ void lz_insert_pass_par(const u8 *ring, u16 *head, u1
 			__syncwarp();
 		}
 	}
-	__syncthreads();
+	bar();
 }
 
 // ---- one chain search (ref: hc_matchfinder.h:182-338) ------------------------------------------
@@ -803,13 +817,14 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 
 	const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 #ifdef LZ_TIMING
-	long long tacc[16] = {};
-	long long tlast = clock64();
+	long long tacc[18] = {};
+	long long tlast = clock64(), tspan = 0;
 #endif
 	const lz_params P = lz_level_params(a.level);
 	// Levels 1-9 (pipe): warps [0, LZ_PWARPS) parse pass k and flush its block while the other warps
 	// search pass k + 1 (nothing the parse and the flush read is written by that search); the last
-	// pass of a chunk, with nothing left to search, is parsed and flushed by the whole CTA.  Levels
+	// pass of a chunk, with nothing left to search, is parsed and flushed by the whole CTA, or by the
+	// first group beside the next chunk's step 0 (the hand-over at the pass loop below).  Levels
 	// 10-12 need the whole block for the min-cost path and run in order on the whole CTA.  GW / GT:
 	// warps / threads of the group that parses and flushes (warp 0 up), gsync() its barrier.
 	const bool pipe = !P.opt_iters;
@@ -821,6 +836,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 
 	if (tid == 0) {
 		v->tma_phase = 0;
+		v->prefetched = 0;
 #ifndef LDB_EMU
 		u32 mbar = (u32)__cvta_generic_to_shared(&v->mbar);
 		asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar) : "memory");
@@ -830,10 +846,12 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 	__syncthreads();
 
 	for (;;) {
-		if (tid == 0) v->chunk = atomicAdd(a.work_counter, 1u);
+		if (tid == 0 && !v->prefetched) v->chunk = atomicAdd(a.work_counter, 1u);
 		__syncthreads();
 		const size_t c = v->chunk;
+		const bool pre = v->prefetched == 2;	// step 0 already ran, beside the previous chunk's last step
 		__syncthreads();
+		if (tid == 0) v->prefetched = 0;
 		if (c >= a.n) break;
 
 		// A piece of a larger stream works in a frame that starts 'dict' bytes before its own input: those
@@ -883,9 +901,9 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		const u32 n = (u32)n64 + dict;	// end of the frame
 		in -= dict;
 
-		// ---- per-chunk init ---------------------------------------------------------------
-		for (u32 i = tid; i < (1u << LZ_HASH_BITS) / 2; i += LZ_THREADS) ((u32 *)head)[i] = 0xffffffffu;
+		// ---- per-chunk init (head[] is reset by step 0) -------------------------------------
 		if (tid == 0) {
+			if (pre) { v->min_len = v->nx_min_len; v->far4_dist = v->nx_far4; }
 			v->failed = 0;
 			v->parse_entry = dict;
 			if (PIECES) { v->dict = dict; v->nonfinal = !final_piece; }
@@ -1249,21 +1267,20 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			gsync();
 		};
 
-		u32 loaded_end = 0;
+		u32 loaded_end = pre ? (n < 2 * LZ_PASS + 16 ? n : 2 * LZ_PASS + 16) : 0;	// (what step 0 loaded)
 		u32 block_begin = dict;
 		u32 block_entry = dict;	// position of the first token of the current block
 		u32 pass_in_block = 0;
 
 		// ---- guided search of pass [b0, pend) -> rs[] (levels 1-9; any set of threads, any number of
 		// times: runs are handed out by v->run_counter and each run's results depend on the run alone)
-		auto search_pass = [&](const u32 b0, const u32 pend, u32 *rs) {
+		auto search_pass = [&](const u32 b0, const u32 pend, u32 *rs, const u32 nn, const u32 min_len, const u32 far4) {
 			// (c) guided search.  Every searcher owns a run of consecutive positions and walks
 			// it like the reference's lazy parser (deflate_compress.c:2605-2808): search where
 			// a token could start, look one position ahead, then skip the positions the
 			// chosen match covers (they inherit it at the same distance).  Every position
 			// still gets a (length, distance), so the exact parallel parse below can start a
 			// token anywhere.  One search call site per loop trip keeps the warp converged.
-			const u32 min_len = v->min_len, far4 = v->far4_dist;
 			// A run starts its walk without knowing where the parse really enters it, so short
 			// runs cost a little ratio (L6: +0.9 % at 16 vs 32) and buy parallelism; the deep
 			// levels, which are chosen for ratio, keep 32.
@@ -1295,14 +1312,14 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 #if LZ_QUANTUM
 					const u32 p0 = b0 + i;
 					wk.best_len = 0; wk.best_dist = 0; wk.left = 0;
-					if (p0 + 4 <= n) {
+					if (p0 + 4 <= nn) {
 						u32 sL = 0, sD = 0;
 						if (pending) { sL = pL - pending >= 4 ? pL - pending : 0; sD = pD; }
-						lz_walk_setup(ring, nextt, p0, n, P.depth >> pending, (u32)P.nice, sL, sD, wk);
+						lz_walk_setup(ring, nextt, p0, nn, P.depth >> pending, (u32)P.nice, sL, sD, wk);
 					}
 					in_search = true;
 				}
-				lz_walk_steps(ring, nextt, b0 + i, n, (u32)P.nice, wk, LZ_QUANTUM);
+				lz_walk_steps(ring, nextt, b0 + i, nn, (u32)P.nice, wk, LZ_QUANTUM);
 				if (wk.left > 0) continue;		// the others move on; this search resumes next trip
 				in_search = false;
 				const u32 p = b0 + i;
@@ -1310,9 +1327,9 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 #else
 				const u32 p = b0 + i;
 				u32 L = 0, D = 0;
-				if (p + 4 <= n) {
+				if (p + 4 <= nn) {
 					if (pending) { L = pL - pending >= 4 ? pL - pending : 0; D = pD; }	// the pending match continues here
-					lz_search(ring, nextt, p, n, P.depth >> pending, (u32)P.nice, L, D);
+					lz_search(ring, nextt, p, nn, P.depth >> pending, (u32)P.nice, L, D);
 				}
 #endif
 				rs[i] = L ? L | ((D - 1) << 16) : 0;
@@ -1354,7 +1371,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 						const u32 pk = b0 + k;
 						// (the match ended on a mismatch unless it was capped at 258 bytes)
 						if (mL == 258)
-							while (mend < n && mend - pk < 258 && lz_ld8(ring, mend) == lz_ld8(ring, mend - mD)) mend++;
+							while (mend < nn && mend - pk < 258 && lz_ld8(ring, mend) == lz_ld8(ring, mend - mD)) mend++;
 						u32 lk = mend - pk;
 						rs[k] = lk >= 4 ? lk | ((mD - 1) << 16) : 0;
 					}
@@ -1833,56 +1850,135 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		// link slots of pass k + 2: insert(k + 1) used them as list scratch and is done with them, and no
 		// chain of pass k + 1 reaches that far back (they belong to positions >= 48 Ki back).
 		// (the passes of the dictionary, step < LZ_DICT / LZ_PASS, are only loaded and inserted)
+		// ---- final partial byte + trailer, by the group [0, GT); a chunk that did not fit gets size 0
+		auto finish = [&]() {
+			if (v->failed) {
+				if (tid == 0) a.out_nbytes[c] = 0;
+				return;
+			}
+			u64 w0 = o.obit >> 5;
+			for (u32 k = tid; k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
+			gsync();
+			if (tid == 0) stage[0] = v->carry;
+			gsync();
+			u64 ob;
+			if (!LZ_NONFINAL) {
+				ob = (o.obit + 7) & ~(u64)7;	// pad the last byte with zero bits
+				if (tid == 0 && trailer) {
+					u8 t[8];
+					def_write_trailer(t, a.format, a.checksums ? a.checksums[c] : 0, n64);
+					for (u32 k = 0; k < trailer; k++) lz_stage_or(stage, (u32)(ob - (w0 << 5)) + 8 * k, t[k], 8);
+				}
+				ob += (u64)trailer * 8;
+			} else {
+				// empty stored block (BFINAL 0, BTYPE 00, zero pad, LEN 0000, NLEN FFFF): the piece ends on a byte
+				ob = (o.obit + 3 + 7) & ~(u64)7;
+				if (tid == 0) lz_stage_or(stage, (u32)(ob - (w0 << 5)), 0xffff0000u, 32);
+				ob += 32;
+			}
+			gsync();
+			u64 bytes_begin = w0 * 4, bytes_end = ob >> 3;
+			for (u64 k = bytes_begin + tid; k < bytes_end; k += GT) {
+				u32 rel = (u32)(k - bytes_begin);
+				o.out[k] = (u8)(stage[rel >> 2] >> (8 * (rel & 3)));
+			}
+			if (tid == 0) a.out_nbytes[c] = (size_t)(ob >> 3);
+		};
+
+		// Hand-over (levels 1-9, batch instance): a chunk of 4k passes (64 KiB, 128 KiB, ...) parses its last
+		// pass in ring slots [48 Ki, 64 Ki), clear of the [0, 32 Ki + 16) that a chunk's step 0 loads.  Its
+		// step npass - 1 fetches the next chunk's index; if that chunk takes the LZ path, the last step runs
+		// on warps [0, LZ_PWARPS) (parse, flush, trailer) while the other warps run the next chunk's step 0
+		// (head reset, loads, min_len, insert(0)) under their own barrier, then search its pass 0; the first
+		// group joins that search once insert(0) is done (bar.arrive / bar.sync).  Owners in that step: the
+		// parse writes its step table into its own pass's link slots (region 3; its search is over), the
+		// insertion its count matrix into region 2 instead of R, which the flush holds; min_len / far4_dist
+		// of the next chunk go to nx_min_len / nx_far4, and its output state (failed, parse_entry,
+		// tok_count, carry, freq) is set up after the join.  res[] parities cannot clash: the last pass
+		// (4k - 1) is odd, pass 0 even.
 		const u32 npass = (n + LZ_PASS - 1) / LZ_PASS;
-		for (u32 step = 0; step < npass + (pipe ? 1 : 0); step++) {
+		const bool hand_on = pipe && !PIECES && (npass & 3) == 0;
+		bool handed = false;
+		for (u32 step = pre ? 1 : 0; step < npass + (pipe ? 1 : 0); step++) {
 			const u32 b0 = step * LZ_PASS;
 			const u32 pend = b0 + LZ_PASS < n ? b0 + LZ_PASS : n;
-			if (step < npass) {
-				if (tid == 0) v->run_counter = 0;
-				__syncthreads();
+			LZ_TSPAN_BEGIN();
+			// last step: does the next chunk (fetched by step npass - 1) start beside it?
+			size_t c1 = 0;
+			u32 n1 = 0;
+			bool beside = false;
+			if (hand_on && step == npass) {
+				c1 = v->chunk;
+				if (c1 < a.n) {
+					const size_t m64 = a.in_nbytes[c1];
+					n1 = (u32)m64;
+					beside = !(m64 <= (size_t)(55 - 4 * a.level) || m64 > 0x7fff0000u) && !(overhead && a.out_avail[c1] <= overhead);
+				}
+			}
+			const bool sg = beside && warp >= LZ_PWARPS;	// this thread runs the next chunk's step 0
+			if (step < npass || sg) {
+				// group of this step's loads and insertion: the whole CTA, or the search group
+				const u32 gt = sg ? tid - 32 * LZ_PWARPS : tid, gw = sg ? LZ_WARPS - LZ_PWARPS : LZ_WARPS, gn = 32 * gw;
+				auto gbar = [&]() {
+					if (sg) LDB_BAR_SYNC(LZ_BAR_S, LZ_THREADS - 32 * LZ_PWARPS);
+					else __syncthreads();
+				};
+				const u8 *src = sg ? (const u8 *)a.in_ptrs[c1] : in;
+				const u32 fn = sg ? n1 : n, fb0 = sg ? 0 : b0, fpend = sg ? (n1 < LZ_PASS ? n1 : LZ_PASS) : pend;
+				if (sg) loaded_end = 0;
+				if (gt == 0) {
+					v->run_counter = 0;
+					if (hand_on && step + 1 == npass) { v->chunk = atomicAdd(a.work_counter, 1u); v->prefetched = 1; }
+				}
+				if (fb0 == 0)
+					for (u32 i = gt; i < (1u << LZ_HASH_BITS) / 2; i += gn) ((u32 *)head)[i] = 0xffffffffu;
+				gbar();
 				// (a) window staging by the TMA engine, one pass ahead: searching this pass needs
 				// [b0 - MAX_DIST, pend + LOOKAHEAD), inserting the next one (concurrently) needs the
 				// bytes up to pend + PASS + 3.  The ring then still holds everything back to
 				// b0 - 32768 + 16, i.e. the whole MAX_DIST window.
 				{
-					const u32 want = pend + LZ_PASS + 16 < n ? pend + LZ_PASS + 16 : n;
+					const u32 want = fpend + LZ_PASS + 16 < fn ? fpend + LZ_PASS + 16 : fn;
 					while (loaded_end < want) {
 						u32 room = LZ_RING - (loaded_end & (LZ_RING - 1));	// a segment must not wrap
 						u32 to = loaded_end + (room < LZ_SEG ? room : LZ_SEG);
 						if (to > want) to = want;
-						lz_load_segment(sm, v, in, loaded_end, to);
+						lz_load_segment(sm, v, src, loaded_end, to, gt, gn, gbar);
 						loaded_end = to;
 					}
 				}
-				if (b0 == LZ_DICT) {
+				if (fb0 == LZ_DICT) {
 					// alphabet size of the first 4 KiB of the chunk's own input -> minimum match length
 					// (ref: calculate_min_match_len, lib/deflate_compress.c:2329-2346)
-					if (tid < 8) { v->used_lits[tid] = 0; v->obs_blk[tid] = 0; }
-					__syncthreads();
-					lz_observe(ring, b0, pend, v->obs_blk, tid, lane, LZ_THREADS);
-					const u32 own = n - LZ_DICT, scan = own < 4096 ? own : 4096;
-					for (u32 i = tid; i < scan; i += LZ_THREADS) {
-						u32 bv = ring[(b0 + i) & (LZ_RING - 1)];
+					if (gt < 8) { v->used_lits[gt] = 0; v->obs_blk[gt] = 0; }
+					gbar();
+					lz_observe(ring, fb0, fpend, v->obs_blk, gt, lane, gn);
+					const u32 own = fn - LZ_DICT, scan = own < 4096 ? own : 4096;
+					for (u32 i = gt; i < scan; i += gn) {
+						u32 bv = ring[(fb0 + i) & (LZ_RING - 1)];
 						atomicOr(&v->used_lits[bv >> 5], 1u << (bv & 31));
 					}
-					__syncthreads();
-					if (tid == 0) {
+					gbar();
+					if (gt == 0) {
 						u32 cnt = 0;
 						for (int k = 0; k < 8; k++) cnt += __popc(v->used_lits[k]);
-						v->min_len = own < 512 ? 4 : lz_choose_min_len(cnt, (u32)P.depth);
+						(sg ? v->nx_min_len : v->min_len) = own < 512 ? 4 : lz_choose_min_len(cnt, (u32)P.depth);
 						// few distinct byte values = cheap literals (text): a far 4-byte match loses against them
-						v->far4_dist = cnt < 80 ? LZ_FAR4_DIST : LZ_WIN;
+						(sg ? v->nx_far4 : v->far4_dist) = cnt < 80 ? LZ_FAR4_DIST : LZ_WIN;
 					}
-					__syncthreads();
+					gbar();
 				}
-				// (b) the whole CTA links this pass into the hash chains (ordered within a hash)
+				// (b) the group links this pass into the hash chains (ordered within a hash)
 				LZ_T(0);	// loads + first-pass extras
+				u32 *cmat = sg ? (u32 *)(nextt + 2 * LZ_PASS) : (u32 *)(sm + LZ_SM_R);
 #ifdef LZ_TIMING
-				lz_insert_pass_par(ring, head, nextt, (u32 *)(sm + LZ_SM_R), b0, pend, n, tid, lane, warp, tacc, tlast);
+				lz_insert_pass_par(ring, head, nextt, cmat, fb0, fpend, fn, gt, lane, warp - (sg ? LZ_PWARPS : 0), gw, gbar, tacc, tlast);
 #else
-				lz_insert_pass_par(ring, head, nextt, (u32 *)(sm + LZ_SM_R), b0, pend, n, tid, lane, warp);
+				lz_insert_pass_par(ring, head, nextt, cmat, fb0, fpend, fn, gt, lane, warp - (sg ? LZ_PWARPS : 0), gw, gbar);
 #endif
 				LZ_T(3);	// insertion: linking
+				if (step == 0) LZ_TSPAN_END(17);
+				if (sg) LDB_BAR_ARRIVE(LZ_BAR_H, LZ_THREADS);	// the parse/flush group may join the search of pass 0
 			}
 			if (!pipe) {
 				if (PIECES && step < v->dict / LZ_PASS) continue;	// (the insertion ended on a CTA barrier)
@@ -1903,87 +1999,67 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				LZ_T(1);	// search phase (barrier to barrier)
 				parse_and_flush(b0, pend, pass_in_block * LZ_PASS, nextt + ((b0 + LZ_PASS) & 0xffff));
 			} else {
-				GW = step < npass ? LZ_PWARPS : LZ_WARPS;
+				GW = step < npass || beside ? LZ_PWARPS : LZ_WARPS;
 				GT = 32 * GW;
 				if (tid < GT && step > LZ_DICT / LZ_PASS) {
 					const u32 kb0 = b0 - LZ_PASS;
-					parse_and_flush(kb0, kb0 + LZ_PASS < n ? kb0 + LZ_PASS : n, ((step - 1) & 1) * LZ_PASS, nextt + ((kb0 + 2 * LZ_PASS) & 0xffff));
+					parse_and_flush(kb0, kb0 + LZ_PASS < n ? kb0 + LZ_PASS : n, ((step - 1) & 1) * LZ_PASS,
+							nextt + ((kb0 + (beside ? 0 : 2 * LZ_PASS)) & 0xffff));
+					if (beside) {
+						finish();
+						LDB_BAR_SYNC(LZ_BAR_H, LZ_THREADS);	// the next chunk's insert(0) is done
+					}
 				}
-				if (step < npass && (!PIECES || step >= v->dict / LZ_PASS)) search_pass(b0, pend, res + (step & 1) * LZ_PASS);
+				if ((step < npass && (!PIECES || step >= v->dict / LZ_PASS)) || beside)
+					search_pass(beside ? 0 : b0, beside ? (n1 < LZ_PASS ? n1 : LZ_PASS) : pend, res + (beside ? 0 : (step & 1) * LZ_PASS),
+						    beside ? n1 : n, beside ? v->nx_min_len : v->min_len, beside ? v->nx_far4 : v->far4_dist);
 				LZ_T(1);	// search (parse/flush group: its share of the search)
 				if (tid == 0) {
 					v->obit_lo = (u32)o.obit; v->obit_hi = (u32)(o.obit >> 32);
 					v->blk_begin = block_begin; v->blk_entry = block_entry; v->blk_passes = pass_in_block;
 				}
+				if (beside && tid == 32 * LZ_PWARPS) v->prefetched = 2;
 			}
 			__syncthreads();
 			LZ_T(14);	// wait at the join
+			if (step == npass) LZ_TSPAN_END(16);
+			if (beside) { handed = true; break; }
 			if (v->failed) break;
 			if (pipe) {	// (every thread takes part in the next whole-CTA parse and flush)
 				o.obit = v->obit_lo | ((u64)v->obit_hi << 32);
 				block_begin = v->blk_begin; block_entry = v->blk_entry; pass_in_block = v->blk_passes;
 			}
 		}
+		if (handed) continue;	// the trailer is written and the next chunk has begun
 		__syncthreads();
-		if (v->failed) {
-			if (tid == 0) a.out_nbytes[c] = 0;
-			__syncthreads();
-			continue;
-		}
-		// ---- final partial byte + trailer ------------------------------------------------
-		{
-			u64 w0 = o.obit >> 5;
-			for (u32 k = tid; k < LZ_STAGE_WORDS; k += LZ_THREADS) stage[k] = 0;
-			__syncthreads();
-			if (tid == 0) stage[0] = v->carry;
-			__syncthreads();
-			u64 ob;
-			if (!LZ_NONFINAL) {
-				ob = (o.obit + 7) & ~(u64)7;	// pad the last byte with zero bits
-				if (tid == 0 && trailer) {
-					u8 t[8];
-					def_write_trailer(t, a.format, a.checksums ? a.checksums[c] : 0, n64);
-					for (u32 k = 0; k < trailer; k++) lz_stage_or(stage, (u32)(ob - (w0 << 5)) + 8 * k, t[k], 8);
-				}
-				ob += (u64)trailer * 8;
-			} else {
-				// empty stored block (BFINAL 0, BTYPE 00, zero pad, LEN 0000, NLEN FFFF): the piece ends on a byte
-				ob = (o.obit + 3 + 7) & ~(u64)7;
-				if (tid == 0) lz_stage_or(stage, (u32)(ob - (w0 << 5)), 0xffff0000u, 32);
-				ob += 32;
-			}
-			__syncthreads();
-			u64 bytes_begin = w0 * 4, bytes_end = ob >> 3;
-			for (u64 k = bytes_begin + tid; k < bytes_end; k += LZ_THREADS) {
-				u32 rel = (u32)(k - bytes_begin);
-				o.out[k] = (u8)(stage[rel >> 2] >> (8 * (rel & 3)));
-			}
-			if (tid == 0) a.out_nbytes[c] = (size_t)(ob >> 3);
-		}
+		GW = LZ_WARPS;
+		GT = LZ_THREADS;
+		finish();
 		__syncthreads();
 		LZ_T(7);	// chunk prologue/epilogue
 	}
 #ifdef LZ_TIMING
 	if (tid == 0 || tid == 32 * LZ_PWARPS)
-		for (int k = 0; k < 15; k++) atomicAdd(&ldb_lz_timing[tid != 0][k], (unsigned long long)tacc[k]);
+		for (int k = 0; k < 18; k++) atomicAdd(&ldb_lz_timing[tid != 0][k], (unsigned long long)tacc[k]);
 #endif
 }
 
 #ifdef LZ_TIMING
 extern "C" __attribute__((visibility("default"))) void ldb_lz_timing_dump(void)
 {
-	unsigned long long h[2][16], z[2][16] = {};
+	unsigned long long h[2][18], z[2][18] = {};
 	cudaDeviceSynchronize();
 	cudaMemcpyFromSymbol(h, ldb_lz_timing, sizeof(h));
 	cudaMemcpyToSymbol(ldb_lz_timing, z, sizeof(z));
-	const char *names[16] = {"loads+first", "search", "parse e5", "insert: linking", "huffman", "precode", "cost+emit", "chunk pro/epilogue",
-				 "parse e1 steps", "parse e2 walks", "parse e3 exit", "parse e4", "insert: hashing", "insert: slice lists", "wait at join", ""};
+	const char *names[18] = {"loads+first", "search", "parse e5", "insert: linking", "huffman", "precode", "cost+emit", "chunk pro/epilogue",
+				 "parse e1 steps", "parse e2 walks", "parse e3 exit", "parse e4", "insert: hashing", "insert: slice lists", "wait at join", "",
+				 "(span) last step", "(span) step 0 load+insert"};
 	const char *who[2] = {"thread 0 (parse/flush group; levels 10-12: whole CTA)", "first thread of the search group"};
 	for (int g = 0; g < 2; g++) {
 		unsigned long long tot = 0;
 		for (int k = 0; k < 15; k++) tot += h[g][k];
 		printf("  timing, clocked by %s:\n", who[g]);
-		for (int k = 0; k < 16; k++)
+		for (int k = 0; k < 18; k++)
 			if (h[g][k]) printf("  timing %-26s %14llu cycles  %5.1f%%\n", names[k], h[g][k], 100.0 * (double)h[g][k] / (double)tot);
 	}
 }

@@ -16,12 +16,14 @@
 #define LDB_SPIN_PAUSE() __nanosleep(100)
 // barrier 'id' (1..15) over the first 'nthreads' threads that reach it (a multiple of 32)
 #define LDB_BAR_SYNC(id, nthreads) asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory")
+// counts the calling threads towards barrier 'id' without waiting (the producer side of bar.sync)
+#define LDB_BAR_ARRIVE(id, nthreads) asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory")
 #else
 #define LDB_SPIN_PAUSE() emu::yield()	// cooperative fibers: a spin loop must hand over
 // bar.sync id, nthreads on the emulator's fibers.  All fibers of a block run on one OS thread, one
 // block after the other, so thread-local counters are the block's own; every barrier completes
 // before its block ends, which leaves them at zero for the next block.
-static inline void ldb_emu_bar_sync(unsigned id, unsigned nthreads)
+static inline void ldb_emu_bar_sync(unsigned id, unsigned nthreads, bool wait = true)
 {
 	static thread_local unsigned arrived[16], gen[16];
 	if (id == 0 || id >= 16 || nthreads == 0 || nthreads % 32 || nthreads > emu::tl_block->nthreads) {
@@ -33,11 +35,12 @@ static inline void ldb_emu_bar_sync(unsigned id, unsigned nthreads)
 		arrived[id] = 0;
 		gen[id]++;
 		emu::tl_block->spins = 0;
-	} else {
+	} else if (wait) {
 		while (gen[id] == mygen) emu::yield();
 	}
 }
 #define LDB_BAR_SYNC(id, nthreads) ldb_emu_bar_sync((id), (nthreads))
+#define LDB_BAR_ARRIVE(id, nthreads) ldb_emu_bar_sync((id), (nthreads), false)
 #endif
 
 typedef uint8_t u8;
