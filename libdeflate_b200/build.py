@@ -77,7 +77,7 @@ def build_emu(force=False):
     objs = []
     procs = []
     common = ["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-DLDB_EMU", "-I", EMU_DIR, "-include", "cuda_emu.h",
-              "-Wno-unused-function", "-fno-strict-aliasing"] + os.environ.get("LDB_EMU_DEFS", "").split()	# (-D switches of a tuning variant)
+              "-Wno-unused-function", "-fno-strict-aliasing"] + os.environ.get("LDB_EMU_DEFS", "").split()	# (-D switches of an instrumented build, e.g. -DINF_STATS)
     for src in SOURCES:
         obj = os.path.join(os.path.dirname(EMU_LIB), src.replace(".cu", ".emu.o"))
         procs.append(subprocess.Popen(common + ["-x", "c++", "-c", os.path.join(CSRC, src), "-o", obj]))

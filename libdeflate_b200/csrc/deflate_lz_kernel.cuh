@@ -41,18 +41,13 @@
 // Algorithmic HBM bytes per chunk: in_nbytes (read once) + out_nbytes (written once).
 #pragma once
 
-#ifndef LZ_THREADS
 #define LZ_THREADS   1024
-#endif
 #define LZ_WARPS     (LZ_THREADS / 32)
 #define LZ_PASS      16384			// positions matched + parsed per pass
 #define LZ_BLOCK_PASSES 2			// passes per DEFLATE block (32 KiB of input)
 #define LZ_NWIN      (LZ_PASS / 32)
-#define LZ_NSL_BITS  (LZ_WARPS >= 32 ? 5 : 4)	// hash slices of the insertion = linking warps
+#define LZ_NSL_BITS  5				// hash slices of the insertion = linking warps
 #define LZ_NSL       (1 << LZ_NSL_BITS)
-#ifndef LZ_QUANTUM
-#define LZ_QUANTUM   0			// > 0: chain steps per loop trip of the resumable search (experiment)
-#endif
 #define LZ_SEG       16384			// largest single TMA load
 #define LZ_RING      65536
 #define LZ_HASH_BITS 13
@@ -69,15 +64,12 @@
 // the 320-symbol alphabets and of the <= 320 code lengths the precode run-length codes.  Deflate
 // kernel at L6, 65536 x 64 KiB, with the speculative-walk parse, on an H100 80GB HBM3 at 700 W:
 // 10 / 12 / 14 warps 262.1 / 258.8 / 266.4 ms.
-#ifndef LZ_PWARPS
 #define LZ_PWARPS    12
-#endif
 #define LZ_BAR_P     1				// named barrier of the parse/flush group
 #define LZ_BAR_S     2				// named barrier of the search group (a chunk's step 0 beside the last step of the one before)
 #define LZ_BAR_H     3				// hand-over: the search group arrives when that step 0 has inserted pass 0
-#ifndef LZ_PF
 #define LZ_PF        4				// parse: windows of per-position results in flight per warp
-#endif
+#define LZ_RUN_SHORT 16				// search: positions per run below level 7 (see search_pass)
 // parse: speculative walk rounds before one thread finishes the pass in order (adversarial inputs)
 #ifndef LZ_SPEC_ROUNDS
 #define LZ_SPEC_ROUNDS 4
@@ -159,10 +151,7 @@ __device__ __forceinline__ lz_params lz_level_params(int level)
 	case 3: return {8, 32, 0, 0};
 	case 4: return {12, 48, 0, 0};
 	case 5: return {12, 48, 1, 0};
-#ifndef LZ_L6_DEPTH
-#define LZ_L6_DEPTH 24
-#endif
-	case 6: return {LZ_L6_DEPTH, 96, 1, 0};
+	case 6: return {24, 96, 1, 0};
 	case 7: return {48, 160, 1, 0};
 	case 8: return {96, 258, 2, 0};		// lazy2: one more position of lookahead (ref: deflate_compress.c:2742-2776)
 	case 9: return {200, 258, 2, 0};
@@ -536,63 +525,6 @@ __device__ __forceinline__ void lz_search(const u8 *ring, const u16 *nextt, u32 
 			if (len >= nice) break;
 			tailo = len - 3;
 			tailv = lz_ld32(ring, p + tailo);
-		}
-	}
-}
-
-// ---- the same search, resumable: a walk is set up once and advanced a few chain steps at a time, so that
-// a lane with a deep chain does not hold back the lanes of its warp that are already done (LZ_QUANTUM > 0)
-struct lz_walk {
-	u32 cand, prev_dist, best_len, best_dist, tailo, tailv, cur;
-	int left;		// chain steps this search may still take (0: finished)
-};
-
-__device__ __forceinline__ void lz_walk_setup(const u8 *ring, const u16 *nextt, u32 p, u32 n, int depth, u32 nice_level,
-					       u32 L, u32 D, lz_walk &w)
-{
-	const u32 max_len = n - p < 258 ? n - p : 258;
-	const u32 nice = nice_level < max_len ? nice_level : max_len;
-	w.best_len = L;
-	w.best_dist = D;
-	if (w.best_len)
-		while (w.best_len < max_len && lz_ld8(ring, p + w.best_len) == lz_ld8(ring, p - w.best_dist + w.best_len)) w.best_len++;
-	w.left = w.best_len >= nice ? 0 : depth;
-	w.cur = lz_ld32(ring, p);
-	w.tailo = w.best_len >= 4 ? w.best_len - 3 : 0;
-	w.tailv = w.tailo ? lz_ld32(ring, p + w.tailo) : w.cur;
-	w.cand = nextt[p & 0xffff];
-	w.prev_dist = 0;
-}
-
-__device__ __forceinline__ void lz_walk_steps(const u8 *ring, const u16 *nextt, u32 p, u32 n, u32 nice_level, lz_walk &w, int quantum)
-{
-	const u32 max_len = n - p < 258 ? n - p : 258;
-	const u32 nice = nice_level < max_len ? nice_level : max_len;
-	const u32 lim = p < LZ_MAX_DIST ? p : LZ_MAX_DIST;
-	for (int q = 0; q < quantum && w.left > 0; q++) {
-		const u32 dist = (p - w.cand) & 0xffff;
-		if (dist - 1 >= lim || dist <= w.prev_dist) { w.left = 0; break; }
-		w.left--;
-		w.prev_dist = dist;
-		const u32 cq = w.cand;
-		w.cand = nextt[cq];
-		if (lz_ld8(ring, cq + w.tailo + 3) != (w.tailv >> 24)) continue;
-		if (lz_ld32(ring, cq + w.tailo) != w.tailv) continue;
-		if (w.tailo && lz_ld32(ring, cq) != w.cur) continue;
-		u32 len = 4;
-		while (len + 4 <= max_len) {
-			u32 x = lz_ld32(ring, p + len) ^ lz_ld32(ring, cq + len);
-			if (x) { len += (__ffs(x) - 1) >> 3; goto extended; }
-			len += 4;
-		}
-		while (len < max_len && lz_ld8(ring, p + len) == lz_ld8(ring, cq + len)) len++;
-	extended:
-		if (len > w.best_len) {
-			w.best_len = len;
-			w.best_dist = dist;
-			if (len >= nice) { w.left = 0; break; }
-			w.tailo = len - 3;
-			w.tailv = lz_ld32(ring, p + w.tailo);
 		}
 	}
 }
@@ -1284,24 +1216,13 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			// A run starts its walk without knowing where the parse really enters it, so short
 			// runs cost a little ratio (L6: +0.9 % at 16 vs 32) and buy parallelism; the deep
 			// levels, which are chosen for ratio, keep 32.
-#ifndef LZ_RUN_SHORT
-#define LZ_RUN_SHORT 16
-#endif
 			const u32 run_len = a.level >= 7 ? 32 : LZ_RUN_SHORT;
 			// runs are handed out dynamically (shared counter): lanes whose runs are cheap
 			// (long matches, few searches) take more of them, which keeps the warp busy
 			u32 i = 0, i_end = 0;
 			u32 pL = 0, pD = 0;		// pending match at position i-pending (lazy evaluation in progress)
 			u32 pending = 0;		// 0: none, 1: looking one position ahead, 2: two positions (lazy2)
-#if LZ_QUANTUM
-			lz_walk wk;
-			wk.left = 0; wk.best_len = 0; wk.best_dist = 0; wk.cand = 0; wk.prev_dist = 0; wk.tailo = 0; wk.tailv = 0; wk.cur = 0;
-			bool in_search = false;
-#endif
 			for (;;) {
-#if LZ_QUANTUM
-				if (!in_search) {
-#endif
 				if (i >= i_end || b0 + i >= pend) {
 					const u32 r = atomicAdd(&v->run_counter, 1u);
 					i = r * run_len;
@@ -1309,29 +1230,12 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					i_end = i + run_len;
 					pending = 0;
 				}
-#if LZ_QUANTUM
-					const u32 p0 = b0 + i;
-					wk.best_len = 0; wk.best_dist = 0; wk.left = 0;
-					if (p0 + 4 <= nn) {
-						u32 sL = 0, sD = 0;
-						if (pending) { sL = pL - pending >= 4 ? pL - pending : 0; sD = pD; }
-						lz_walk_setup(ring, nextt, p0, nn, P.depth >> pending, (u32)P.nice, sL, sD, wk);
-					}
-					in_search = true;
-				}
-				lz_walk_steps(ring, nextt, b0 + i, nn, (u32)P.nice, wk, LZ_QUANTUM);
-				if (wk.left > 0) continue;		// the others move on; this search resumes next trip
-				in_search = false;
-				const u32 p = b0 + i;
-				u32 L = wk.best_len, D = wk.best_dist;
-#else
 				const u32 p = b0 + i;
 				u32 L = 0, D = 0;
 				if (p + 4 <= nn) {
 					if (pending) { L = pL - pending >= 4 ? pL - pending : 0; D = pD; }	// the pending match continues here
 					lz_search(ring, nextt, p, nn, P.depth >> pending, (u32)P.nice, L, D);
 				}
-#endif
 				rs[i] = L ? L | ((D - 1) << 16) : 0;
 				u32 mpos, mL, mD;	// match to accept this trip (mL == 0: none)
 				if (pending) {

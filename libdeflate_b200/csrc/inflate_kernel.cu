@@ -58,22 +58,14 @@
 // is extra traffic of the two-kernel split and is reported as such (bench.py "traffic").
 #include "ldb_common.cuh"
 
-// table geometry (overridable at build time for tuning sweeps, see scripts/build_variants.py)
-#ifndef INF_LB
+// table geometry
 #define INF_LB        7			// main litlen table bits
-#endif
 #define INF_LMAIN     (1 << INF_LB)
-#ifndef INF_LSUB_SM
 #define INF_LSUB_SM   24		// litlen subtable entries kept in shared memory (24, not 32: 16 warps fit an SM)
-#endif
 #define INF_LSUB_CAP  2048		// total litlen subtable capacity (rest in global scratch)
-#ifndef INF_OB
 #define INF_OB        5			// main offset table bits
-#endif
 #define INF_OMAIN     (1 << INF_OB)
-#ifndef INF_OSUB_SM
 #define INF_OSUB_SM   32
-#endif
 #define INF_OSUB_CAP  2048		// a 5-bit root can need a 1024-entry subtable plus smaller ones
 #define INF_L_ENTRIES (INF_LMAIN + INF_LSUB_SM)		// 640 u16 per lane
 #define INF_O_ENTRIES (INF_OMAIN + INF_OSUB_SM)		// 128 u16 per lane
@@ -88,17 +80,8 @@
 #define INF_GS_BYTES   ((INF_GS_LENS + 320 + 127) & ~127)
 
 // the token stream is written once here and read once by the next kernel: cache-streaming stores
-#ifndef INF_STREAM_HINTS
-#define INF_STREAM_HINTS 1
-#endif
-#if INF_STREAM_HINTS
 #define INF_ST_TOK(p, v) __stcs((p), (v))
-#else
-#define INF_ST_TOK(p, v) (*(p) = (v))
-#endif
-#ifndef INF_QUANTUM
 #define INF_QUANTUM   384		// decode steps between service phases
-#endif
 
 // per-warp shared memory layout (bytes)
 #define INF_SM_LTAB    0
@@ -107,23 +90,12 @@
 #define INF_SM_CNT     (INF_SM_SCRATCH)				// u32[16]
 #define INF_SM_CODE    (INF_SM_CNT + 64)			// u32[16]
 #define INF_SM_SUBBITS (INF_SM_CODE + 64)			// u8[1 << INF_LB]
-#ifndef INF_FUSE_OFF
-#define INF_FUSE_OFF 1		// a match's offset is decoded in the same step as its length when both fit
-#endif
-#ifndef INF_LIT2
 #define INF_LIT2 4		// how many literals that follow a literal or a completed match are decoded in the same step
-#endif
 #define INF_SM_WQ      (INF_SM_SUBBITS + (1 << INF_LB))		// u32[32]: per-lane prefetched input word of the decode loop
-#ifndef INF_WQ2
-#define INF_WQ2 0		// 1: two lookahead words per lane, one copy group per step (profiles/r02_inflate_d.md, call P)
-#endif
-#define INF_SM_BYTES   (INF_SM_WQ + 128 + 128 * INF_WQ2)		// per warp: 14208 with the default geometry
-#ifndef INF_WPC
+#define INF_SM_BYTES   (INF_SM_WQ + 128)		// per warp: 14208
 #define INF_WPC        8		// independent warps per CTA
-#endif
 
 static_assert(INF_O_ENTRIES >= 64, "the offset region doubles as the 128-byte precode table scratch");
-static_assert(INF_LB >= INF_OB && INF_LB <= 10 && INF_OB >= 5, "table geometry");
 
 // entry encodings (u16)
 // bits 15..14: 0 literal (value << 4 | codeword bits), 1 "value" symbol = length or offset slot
@@ -170,7 +142,6 @@ struct inf_lane {
 	u32 hlit, hdist, is_static;
 	u32 stored_len, stored_src;
 	u32 pend_len;		// decoded match length whose offset has not been decoded yet (ST_OFF)
-	u32 ri;			// INF_WQ2: which lookahead slot holds the word at wpos + 8
 	// bookkeeping
 	u32 chunk;		// chunk index
 	u32 hdr_bytes;		// wrapper header size
@@ -198,12 +169,7 @@ __device__ __forceinline__ void inf_cp_async4(u32 *smem_dst, const void *gsrc)
 	asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((u32)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
 __device__ __forceinline__ void inf_cp_async_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-__device__ __forceinline__ void inf_cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-// everything but the copies of the most recent group (= the most recent decode step) has landed
-__device__ __forceinline__ void inf_cp_async_wait_older() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 #else
-__device__ __forceinline__ void inf_cp_async_commit() {}
-__device__ __forceinline__ void inf_cp_async_wait_older() {}
 __device__ __forceinline__ void inf_cp_async4(u32 *smem_dst, const void *gsrc) { *smem_dst = *(const u32 *)gsrc; }
 __device__ __forceinline__ void inf_cp_async_wait() {}
 #endif
@@ -791,7 +757,6 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 	const bool is_offv = is_val && isoff;
 	// length: "no room" is decided before the offset is looked at (decompress_template.h:696-701)
 	const bool len_fits = val <= s.lit_limit - s.n_lit;
-#if INF_FUSE_OFF
 	// The offset of a match in the SAME step as its length: after the follow-on literals two of three steps
 	// were the length / offset pairs of matches.  Taken when the offset's codeword sits in the main offset
 	// table and length + offset fit the 32 bits of 'bits' (nearly always); otherwise the next step is an
@@ -803,10 +768,6 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 	const u32 valo = (oslot >= 4 ? 1 + ((2 + (oslot & 1)) << ebo) : 1 + oslot) + ((obits >> clo) & ((1u << ebo) - 1));
 	const bool fuse = is_len && len_fits && eo < LE_SUB_FLAG && adv + clo + ebo <= 32;
 	adv += fuse ? clo + ebo : 0u;
-#else
-	const bool fuse = false;
-	const u32 valo = 0, obits = 0, clo = 0, ebo = 0;
-#endif
 	const u32 m_len = fuse ? val : s.pend_len;
 	const u32 m_off = fuse ? valo : val;
 	const bool have_off = is_offv || fuse;
@@ -829,7 +790,6 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 	s.lit_limit -= emit ? m_len : 0u;
 	const bool len_only = is_len && !fuse;		// the offset follows in the next step
 	s.pend_len = len_only ? val : s.pend_len;
-#if INF_LIT2
 	// A literal FOLLOWING this step's symbol is taken in the same step: 72 % of the bench corpus' symbols are
 	// literals, so after a literal, and after the offset that completes a match, the next main-table entry
 	// is looked up at once and taken if it is a plain literal whose codeword still lies inside the 32 bits of
@@ -854,7 +814,6 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 #endif
 		}
 	}
-#endif
 	s.bitpos += live ? adv : 0u;
 	// next state / verdict (the verdict is only read in ST_DONE)
 	u32 st = s.state, vd = s.verdict;
@@ -880,24 +839,6 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 	// in the lane's shared-memory slot wq: the next word is fetched into it by an asynchronous copy, so the
 	// load is tied to no register (held in a register, the compiler copied the word being loaded into the
 	// loop-carried register at the bottom of the loop and every step waited there: 10 % of the stall samples).
-#if INF_WQ2
-	// Two lookahead words per lane and one copy group per step: a refill waits only for groups older than
-	// the most recent one, and a word is used no earlier than two refills (>= two steps) after it was asked for.
-	inf_cp_async_commit();
-	const bool rf = act && s.bitpos >= 32;
-	if (rf) {
-		inf_cp_async_wait_older();
-		volatile u32 *slot = wq + 32 * s.ri;	// holds the word at wpos + 8
-		s.w0 = s.w1;
-		s.w1 = *slot;
-		s.wpos += 4;
-		s.bitpos -= 32;
-		const u32 pos = s.wpos + 12;		// the other slot holds wpos + 8 now; fetch the word after it
-		if (pos + 4 <= s.in_nal) inf_cp_async4((u32 *)slot, s.in_al + pos);
-		else *slot = inf_ld_word(s, pos);	// ragged end of the input: zero-padded word
-		s.ri ^= 1;
-	}
-#else
 	const bool rf = act && s.bitpos >= 32;
 	if (rf) {
 		inf_cp_async_wait();			// the word asked for ~3 steps ago
@@ -909,16 +850,13 @@ __device__ __forceinline__ void inf_decode_step(inf_lane &s, const u8 *sm, const
 		if (pos + 4 <= s.in_nal) inf_cp_async4(wq, s.in_al + pos);
 		else *(volatile u32 *)wq = inf_ld_word(s, pos);	// ragged end of the input: zero-padded word
 	}
-#endif
 }
 
 // ---- the decode kernel --------------------------------------------------------------
 // The warps of a CTA are independent (each has its own tables and never syncs with the others);
 // INF_WPC of them share a CTA only because shared memory is reserved per CTA (1 KiB each), and
 // 2 CTAs x 8 warps fit where 16 single-warp CTAs would not.
-#ifndef INF_MIN_CTAS
 #define INF_MIN_CTAS 2		// CTAs per SM the register allocation must allow
-#endif
 // Segment mode (SEG, decompress_large): chunk c is a segment of ONE stream, described by g (ldb_common.cuh).
 // The batch instance (SEG = false) compiles to the code it had before the mode existed.
 
@@ -948,7 +886,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 	s.chunk = 0xffffffffu;
 	s.in = nullptr; s.in_al = nullptr; s.in_a0 = 0; s.in_n = 0; s.in_nal = 0; s.wpos = 0; s.w0 = 0; s.w1 = 0; s.w2 = 0; s.bitpos = 0;
 	s.lit = nullptr; s.rec_end = nullptr; s.n_lit = 0; s.n_rec = 0; s.lit_mark = 0; s.lit_limit = 0; s.out_avail = 0; s.acc = 0;
-	s.is_final = 0; s.hlit = 0; s.hdist = 0; s.is_static = 0; s.stored_len = 0; s.stored_src = 0; s.hdr_bytes = 0; s.pend_len = 0; s.ri = 0;
+	s.is_final = 0; s.hlit = 0; s.hdist = 0; s.is_static = 0; s.stored_len = 0; s.stored_src = 0; s.hdr_bytes = 0; s.pend_len = 0;
 	bool exhausted = false;
 
 	// the bookkeeping of a stream that has ended (ST_DONE) with s.verdict; the lane becomes idle
@@ -1227,20 +1165,12 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 #pragma unroll 1
 		u32 *wq = (u32 *)(sm + INF_SM_WQ) + lane;
 		*(volatile u32 *)wq = s.w2;		// inside the loop the third window word lives in shared memory
-#if INF_WQ2
-		s.ri = 0;				// slot[ri] = word at wpos + 8, slot[ri ^ 1] = word at wpos + 12
-		*(volatile u32 *)(wq + 32) = s.state >= ST_LIT ? inf_ld_word(s, s.wpos + 12) : 0;
-#endif
 		for (int it = 0; it < INF_QUANTUM; it++) {
 			inf_decode_step<SEG>(s, sm, ovf, lane, wq);
 			if ((it & 31) == 31 && !__any_sync(LDB_FULL_MASK, s.state >= ST_LIT)) break;
 		}
 		inf_cp_async_wait();
-#if INF_WQ2
-		s.w2 = *(volatile u32 *)(wq + 32 * s.ri);
-#else
 		s.w2 = *(volatile u32 *)wq;		// ... and outside of it in a register again
-#endif
 		__syncwarp();
 	}
 }

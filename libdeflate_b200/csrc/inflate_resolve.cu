@@ -33,24 +33,13 @@
 #define RES_STG     4096u	// staging ring: the group being assembled, position q at q % 4096
 #define RES_SMASK   (RES_STG - 1)
 #define RES_SPAN    2048u	// most output bytes one group of records may cover
-#ifndef RES_LIT_FAST
 #define RES_LIT_FAST 16u	// literal runs up to this are placed by the owning lane in one step
-#endif
 #define RES_SLACK   32u		// bytes behind the ring's end that a piece may run into (res_store16)
 #define RES_SM_BYTES (RES_STG + RES_SLACK)
 // token records are read exactly once: cache-streaming loads (evict-first) keep them from displacing the
 // window rows in L2
-#ifndef RES_STREAM_HINTS
-#define RES_STREAM_HINTS 1
-#endif
-#if RES_STREAM_HINTS
 #define RES_LD_REC(p) __ldcs(p)
-#else
-#define RES_LD_REC(p) __ldg(p)
-#endif
-#ifndef RES_PER_SM
 #define RES_PER_SM  32		// warps (= chunks) per SM: as many as an SM holds CTAs, the walk is latency-bound
-#endif
 
 // the scratch slot of a chunk: what the decoder can emit is bounded both by the output room
 // (a record stands for >= 3 bytes or for up to 2^31 literals) and by the input (a literal takes

@@ -34,6 +34,7 @@ def main():
     db = json.load(open(path)) if os.path.exists(path) else {}
     db[key] = {k: {"dram_bytes_per_launch": sum(v) / len(v), "launches_measured": len(v)} for k, v in out.items()}
     db[key]["source"] = "ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum (scripts/ncu_traffic.py)"
+    os.makedirs(os.path.dirname(path), exist_ok=True)
     json.dump(db, open(path, "w"), indent=1, sort_keys=True)
     print(json.dumps(db[key]))
 
