@@ -11,6 +11,7 @@
 // lib/deflate_compress.c:2393-2443).  The LZ77 + Huffman path is in
 // deflate_lz_kernel.cuh.
 #include <stdlib.h>
+#include <string.h>
 
 #include "ldb_common.cuh"
 
@@ -69,6 +70,27 @@ int ldb_deflate_grid(const ldb_launch_cfg &cfg)
 		if (k > 0 && k < g) g = k;
 	}
 	return g;
+}
+
+// Parse/flush group sizes of the LZ kernel at levels 1-9 (deflate_lz_kernel.cuh, LZ_GROUP_*).
+// LIBDEFLATE_B200_DEFLATE_GROUPS=Q,F,H sets them for tests and tuning: the warps of a step that only
+// parses, of one that also flushes a block, and of a chunk's hand-over step.  Each value is clamped to
+// its legal range; an empty or missing one keeps its default.  Streams do not depend on these sizes.
+void ldb_deflate_groups(int level, u32 pwarps[3])
+{
+	static const u32 parse[9] = LZ_GROUP_PARSE;
+	const u32 def[3] = {level >= 1 && level <= 9 ? parse[level - 1] : LZ_GROUP_FLUSH, LZ_GROUP_FLUSH, LZ_GROUP_HAND};
+	const u32 lo[3] = {LZ_GROUP_MIN_PARSE, LZ_GROUP_MIN_FLUSH, LZ_GROUP_MIN_FLUSH};
+	const char *e = getenv("LIBDEFLATE_B200_DEFLATE_GROUPS");
+	for (int k = 0; k < 3; k++) {
+		pwarps[k] = def[k];
+		if (!e) continue;
+		char *end;
+		const long x = strtol(e, &end, 10);
+		if (end != e) pwarps[k] = x < (long)lo[k] ? lo[k] : (x > LZ_GROUP_MAX ? LZ_GROUP_MAX : (u32)x);
+		e = strchr(end, ',');
+		if (e) e++;
+	}
 }
 
 int ldb_launch_deflate(const ldb_deflate_args &a, const ldb_launch_cfg &cfg, void *stream)

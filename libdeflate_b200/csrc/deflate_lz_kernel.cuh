@@ -59,12 +59,47 @@
 // tokens per thread per emission round of a group of gt threads: <= 1024 tokens of <= 48 bits per
 // round (<= 1536 staging words)
 #define LZ_TPT(gt)     ((gt) > 512 ? 1u : 2u)
-// Levels 1-9 run two warp groups: warps [0, LZ_PWARPS) parse pass k and flush its block while the
-// others search pass k + 1, then join that search.  The block flush needs one thread per symbol of
-// the 320-symbol alphabets and of the <= 320 code lengths the precode run-length codes.  Deflate
-// kernel at L6, 65536 x 64 KiB, with the speculative-walk parse, on an H100 80GB HBM3 at 700 W:
-// 10 / 12 / 14 warps 262.1 / 258.8 / 266.4 ms.
-#define LZ_PWARPS    12
+// Levels 1-9 run two warp groups: warps [0, GW) parse pass k and flush its block while the others
+// search pass k + 1, then join that search.  GW depends on what the step's parse does, which is known
+// before the step splits (the block-end decision is taken during the insertion, from byte classes the
+// last warps counted in the step before): LZ_GROUP_PARSE[level]
+// warps when the block goes on, LZ_GROUP_FLUSH when it ends there, LZ_GROUP_HAND for a chunk's last pass
+// beside the next chunk's step 0.  A flush needs one thread per symbol of the 320-symbol alphabets and
+// of the <= 320 code lengths the precode run-length codes, so >= 10 warps; a parse alone takes any
+// number of warps (windows are dealt out per warp, the scans are one warp's).  The launch may override
+// the defaults within [min, LZ_GROUP_MAX] (ldb_deflate_groups).  Deflate kernel at L6, 65536 x 64 KiB
+// gzip, on an H100 80GB HBM3 at 700 W (scripts/sweep_deflate_groups.py, medians of 2 rounds, ms):
+//            F=12   F=14   F=16   F=18   F=20   F=24      (H = 12; H = 16 adds 8.5-9 ms to every cell)
+//     Q=4   250.5  251.1  253.9  258.6  264.4  268.6
+//     Q=6   241.1  241.6  244.4  249.4  256.6  258.9
+//     Q=8   242.7  243.2  246.0  250.8  256.6  260.7
+//     Q=10  244.3  244.8  247.7  252.4  258.0  262.3
+//     Q=12  250.7  251.0  253.8  258.9  264.5  268.5
+// Q 5-7, F 10-12, H 10-12: best (5, 12, 10) 238.3 ms, (6, 12, 10) 239.6, (5, 12, 12) 239.6, (6, 12, 12) 241.2; F < 12 costs.
+// The parse-only group by level, F = H = 12, 16384 x 64 KiB, ms (the previous build with 12 warps for
+// every step in the first column):
+//            prev    Q=4    Q=6    Q=8   Q=10   Q=12   Q=14   Q=16
+//     L1    43.89  53.41  48.55  45.77  44.41  43.69  43.60  43.87
+//     L2    44.91  53.40  48.57  45.86  44.81  44.98  45.27  45.70
+//     L3    47.97  54.36  49.62  47.68  47.79  48.04  48.52  49.46
+//     L4    50.02  55.03  50.28  49.61  49.74  50.06  50.63  51.58
+//     L5    54.25  58.94  53.75  53.70  53.90  54.38  56.10  55.83
+//     L6    61.87  62.92  60.55  60.96  61.35  62.96  63.33  63.00
+//     L7    86.87  86.93  86.91  87.15  87.05  86.95  87.05  86.21
+//     L8   122.93 125.88 122.80 122.83 122.94 122.69 122.59 121.63
+//     L9   180.28 179.64 179.79 179.67 180.13 179.42 179.33 177.91
+// A shallow search (L1, L2) is done before a narrow group has parsed, so the parse wants the warps; at
+// L6, 12 warps left the group idle for half of a parse-only step (phase clocks), so 5 give the search
+// more hands; from L7 on, runs of 32 positions (search_pass) leave half the CTA without one and the
+// size hardly matters.  Wider flush and hand-over groups only take warps from the search.
+// (These sweeps ran with the next pass's class count inside the whole-CTA insertion; DESIGN §10.)
+// Before, one size for every step: 10 / 12 / 14 warps 262.1 / 258.8 / 266.4 ms (before the hand-over).
+#define LZ_GROUP_PARSE     {12, 10, 8, 8, 8, 5, 16, 16, 16}	// levels 1-9
+#define LZ_GROUP_FLUSH     12
+#define LZ_GROUP_HAND      10
+#define LZ_GROUP_MIN_PARSE 4
+#define LZ_GROUP_MIN_FLUSH 10
+#define LZ_GROUP_MAX       28			// the search group keeps >= 4 warps
 #define LZ_BAR_P     1				// named barrier of the parse/flush group
 #define LZ_BAR_S     2				// named barrier of the search group (a chunk's step 0 beside the last step of the one before)
 #define LZ_BAR_H     3				// hand-over: the search group arrives when that step 0 has inserted pass 0
@@ -75,7 +110,9 @@
 #define LZ_SPEC_ROUNDS 4
 #endif
 static_assert(LZ_SPEC_ROUNDS >= 1 && LZ_SPEC_ROUNDS <= 14, "round statistic buckets");
-static_assert(LZ_PWARPS >= 10 && LZ_PWARPS < LZ_WARPS, "parse/flush group: 320..LZ_THREADS-32 threads");
+static_assert(LZ_GROUP_MIN_PARSE >= 1 && LZ_GROUP_MIN_FLUSH * 32 >= 320 && LZ_GROUP_MAX < LZ_WARPS, "group size bounds");
+static_assert(LZ_GROUP_FLUSH >= LZ_GROUP_MIN_FLUSH && LZ_GROUP_FLUSH <= LZ_GROUP_MAX && LZ_GROUP_HAND >= LZ_GROUP_MIN_FLUSH &&
+	      LZ_GROUP_HAND <= LZ_GROUP_MAX, "default group sizes");
 
 // shared memory layout
 #define LZ_SM_RING   0
@@ -122,7 +159,7 @@ struct lz_vars {
 	u32 nused_lit, nused_off;
 	u32 huff_over;		// a Huffman code exceeded 15 bits and was capped
 	u32 obs_blk[8], obs_next[8];	// byte-class observations: current block / the pass after it
-	u32 end_early;		// the next pass looks different: end the block before it
+	u32 end_block;		// the block ends with the pass being parsed (lz_end_block_decide)
 	u32 failed;
 	u32 obit_lo, obit_hi;	// output bit position (64-bit) } the parse/flush group's block state, published at
 	u32 blk_begin, blk_entry, blk_passes;	// block_begin, block_entry, pass_in_block  } every join
@@ -337,19 +374,33 @@ __device__ __forceinline__ void lz_gen_codes_serial(const u8 *lens, u32 nsyms, u
 #ifdef LZ_TIMING
 #include <stdio.h>
 // tuning builds only: cycles per phase, summed over all CTAs, clocked separately by thread 0 (first
-// warp of the parse/flush group) and by the first thread of the search group; whole-CTA phases appear
-// in both.  (The compiler may read the clock before a barrier wait, so a phase in which the clocking
-// thread finishes early is under-counted and the wait shows up in the next one.)  Slots 16 and 17 clock
-// whole stretches that the phases 0-14 already cover: a chunk's last step (from its start to its join)
-// and step 0's load and insertion.
-__device__ unsigned long long ldb_lz_timing[2][18];
-#define LZ_T(k) do { if (tid == 0 || tid == 32 * LZ_PWARPS) { long long t_ = clock64(); tacc[k] += t_ - tlast; tlast = t_; } } while (0)
-#define LZ_TSPAN_BEGIN() do { if (tid == 0 || tid == 32 * LZ_PWARPS) tspan = clock64(); } while (0)
-#define LZ_TSPAN_END(k) do { if (tid == 0 || tid == 32 * LZ_PWARPS) tacc[k] += clock64() - tspan; } while (0)
+// warp of the parse/flush group) and by the first thread of the last warp, which is in the search group
+// whatever the group sizes; whole-CTA phases appear in both.  (The compiler may read the clock before a
+// barrier wait, so a phase in which the clocking thread finishes early is under-counted and the wait
+// shows up in the next one.)  Slots 16 and 17 clock whole stretches that the phases 0-14 already cover:
+// a chunk's last step (from its start to its join) and step 0's load and insertion.  Slots 18-29 split
+// the steps in which the two groups run side by side by kind (parse only, parse + block flush, hand-over):
+// the parse/flush group's busy cycles (thread 0), each group's wait at the join, the number of such
+// steps and their span from the split to the join.
+#define LZ_TSLOTS 30
+__device__ unsigned long long ldb_lz_timing[2][LZ_TSLOTS];
+#define LZ_TCLK (tid == 0 || tid == LZ_THREADS - 32)
+#define LZ_T(k) do { if (LZ_TCLK) { long long t_ = clock64(); tacc[k] += t_ - tlast; tlast = t_; } } while (0)
+#define LZ_TSPAN_BEGIN() do { if (LZ_TCLK) tspan = clock64(); } while (0)
+#define LZ_TSPAN_END(k) do { if (LZ_TCLK) tacc[k] += clock64() - tspan; } while (0)
+#define LZ_TSPLIT_BEGIN() do { if (LZ_TCLK) tsplit = clock64(); } while (0)
+#define LZ_TSPLIT_BUSY() do { if (tid == 0) tbusy = clock64() - tsplit; } while (0)
+#define LZ_TJOIN_BEGIN() do { if (LZ_TCLK) tjoin = clock64(); } while (0)
+#define LZ_TSPLIT_END(split, kind) do { if ((split) && LZ_TCLK) { const long long t_ = clock64(); const int k_ = (kind); \
+	tacc[18 + k_] += tbusy; tacc[21 + k_] += t_ - tjoin; tacc[24 + k_] += 1; tacc[27 + k_] += t_ - tsplit; } } while (0)
 #else
 #define LZ_T(k) do { } while (0)
 #define LZ_TSPAN_BEGIN() do { } while (0)
 #define LZ_TSPAN_END(k) do { } while (0)
+#define LZ_TSPLIT_BEGIN() do { } while (0)
+#define LZ_TSPLIT_BUSY() do { } while (0)
+#define LZ_TJOIN_BEGIN() do { } while (0)
+#define LZ_TSPLIT_END(split, kind) do { } while (0)
 #endif
 
 #ifdef LZ_SPEC_STATS
@@ -398,9 +449,11 @@ __device__ __forceinline__ u32 lz_same_key_mask(u32 key, bool valid)
 //      the same-hash lane mask, the others from head[].  Same links as a serial insertion.
 // Run by a group of gw warps (warp: rank in the group, tid: thread rank, bar: its barrier); with fewer
 // warps than slices a warp links several lists in turn, which gives the same links.
-template <typename Bar>
+// decide: one thread of the group's last warp runs decided() beside warp 0's scan (no barrier of its own).
+template <typename Bar, typename Decided>
 __device__ __forceinline__ void lz_insert_pass_par(const u8 *ring, u16 *head, u16 *nextt, u32 *cmat,
-						   u32 b0, u32 pend, u32 n, u32 tid, u32 lane, u32 warp, u32 gw, Bar bar
+						   u32 b0, u32 pend, u32 n, u32 tid, u32 lane, u32 warp, u32 gw, Bar bar,
+						   bool decide, Decided decided
 #ifdef LZ_TIMING
 						   , long long *tacc, long long &tlast
 #endif
@@ -422,6 +475,7 @@ __device__ __forceinline__ void lz_insert_pass_par(const u8 *ring, u16 *head, u1
 	}
 	bar();
 	LZ_T(12);	// insertion: hashing
+	if (decide && tid == 32 * (gw - 1)) decided();
 	if (warp == 0) {
 		u32 run = 0;
 		if (lane < LZ_NSL)
@@ -708,6 +762,19 @@ __device__ __forceinline__ bool lz_should_end_block(const u32 *obs, const u32 *o
 	return total_delta + (u64)(block_length / 4096) * n_old >= cutoff;
 }
 
+// One thread: does the block end with the pass just parsed (its passes so far, its length in bytes), given
+// the classes of the next pass in obs_next?  -> v->end_block.  obs_blk restarts with the next pass's counts
+// when the block ends and accumulates them otherwise; obs_next is cleared for the count of the pass after.
+__device__ __forceinline__ void lz_end_block_decide(lz_vars *v, u32 passes, u32 block_length)
+{
+	const bool end = passes == LZ_BLOCK_PASSES || lz_should_end_block(v->obs_blk, v->obs_next, block_length);
+	v->end_block = end ? 1 : 0;
+	for (int k = 0; k < 8; k++) {
+		v->obs_blk[k] = end ? v->obs_next[k] : v->obs_blk[k] + v->obs_next[k];
+		v->obs_next[k] = 0;
+	}
+}
+
 // ---- the kernel ----------------------------------------------------------------------------
 // PIECES: the launch carries ldb_deflate_args::piece (pieces of one stream).  The batch path is the
 // instance without it, where the dictionary is 0 and every chunk final at compile time.
@@ -749,16 +816,17 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 
 	const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 #ifdef LZ_TIMING
-	long long tacc[18] = {};
-	long long tlast = clock64(), tspan = 0;
+	long long tacc[LZ_TSLOTS] = {};
+	long long tlast = clock64(), tspan = 0, tsplit = 0, tbusy = 0, tjoin = 0;
 #endif
 	const lz_params P = lz_level_params(a.level);
-	// Levels 1-9 (pipe): warps [0, LZ_PWARPS) parse pass k and flush its block while the other warps
+	// Levels 1-9 (pipe): warps [0, GW) parse pass k and flush its block while the other warps
 	// search pass k + 1 (nothing the parse and the flush read is written by that search); the last
 	// pass of a chunk, with nothing left to search, is parsed and flushed by the whole CTA, or by the
 	// first group beside the next chunk's step 0 (the hand-over at the pass loop below).  Levels
 	// 10-12 need the whole block for the min-cost path and run in order on the whole CTA.  GW / GT:
-	// warps / threads of the group that parses and flushes (warp 0 up), gsync() its barrier.
+	// warps / threads of the group that parses and flushes (warp 0 up; per step, a.pwarps), gsync() its
+	// barrier.
 	const bool pipe = !P.opt_iters;
 	u32 GW = LZ_WARPS, GT = LZ_THREADS;
 	auto gsync = [&]() {
@@ -836,6 +904,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		// ---- per-chunk init (head[] is reset by step 0) -------------------------------------
 		if (tid == 0) {
 			if (pre) { v->min_len = v->nx_min_len; v->far4_dist = v->nx_far4; }
+			else for (int k = 0; k < 8; k++) v->obs_next[k] = 0;	// (a step 0 beside the chunk before counted pass 1 already)
 			v->failed = 0;
 			v->parse_entry = dict;
 			if (PIECES) { v->dict = dict; v->nonfinal = !final_piece; }
@@ -1294,19 +1363,19 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			LZ_T(2);	// parse
 			// ---- block boundary: every LZ_BLOCK_PASSES passes, or at the end of the input --------
 			// A block also ends early when the bytes of the next pass look different from the block
-			// so far (the reference's block-split test, on pass granularity).
+			// so far (the reference's block-split test, on pass granularity).  Levels 1-9 decided it while
+			// the next pass was inserted, before the step split; levels 10-12 decide it here.
 			pass_in_block++;
 			if (!last) {
-				if (tid < 8) v->obs_next[tid] = 0;
-				gsync();
-				lz_observe(ring, pend, pend + LZ_PASS < n ? pend + LZ_PASS : n, v->obs_next, tid, lane, GT);
-				gsync();
-				if (tid == 0) v->end_early = lz_should_end_block(v->obs_blk, v->obs_next, pend - block_begin) ? 1 : 0;
-				gsync();
-				const bool end_now = pass_in_block == LZ_BLOCK_PASSES || v->end_early;
-				gsync();
-				if (tid < 8) v->obs_blk[tid] = end_now ? v->obs_next[tid] : v->obs_blk[tid] + v->obs_next[tid];
-				if (!end_now) return;
+				if (!pipe) {
+					if (tid < 8) v->obs_next[tid] = 0;
+					gsync();
+					lz_observe(ring, pend, pend + LZ_PASS < n ? pend + LZ_PASS : n, v->obs_next, tid, lane, GT);
+					gsync();
+					if (tid == 0) lz_end_block_decide(v, pass_in_block, pend - block_begin);
+					gsync();
+				}
+				if (!v->end_block) return;
 			}
 			const u32 npass_block = pass_in_block;
 			pass_in_block = 0;
@@ -1792,7 +1861,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		// Hand-over (levels 1-9, batch instance): a chunk of 4k passes (64 KiB, 128 KiB, ...) parses its last
 		// pass in ring slots [48 Ki, 64 Ki), clear of the [0, 32 Ki + 16) that a chunk's step 0 loads.  Its
 		// step npass - 1 fetches the next chunk's index; if that chunk takes the LZ path, the last step runs
-		// on warps [0, LZ_PWARPS) (parse, flush, trailer) while the other warps run the next chunk's step 0
+		// on warps [0, H) (parse, flush, trailer; H = a.pwarps[2]) while the other warps run the next chunk's step 0
 		// (head reset, loads, min_len, insert(0)) under their own barrier, then search its pass 0; the first
 		// group joins that search once insert(0) is done (bar.arrive / bar.sync).  Owners in that step: the
 		// parse writes its step table into its own pass's link slots (region 3; its search is over), the
@@ -1819,12 +1888,13 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					beside = !(m64 <= (size_t)(55 - 4 * a.level) || m64 > 0x7fff0000u) && !(overhead && a.out_avail[c1] <= overhead);
 				}
 			}
-			const bool sg = beside && warp >= LZ_PWARPS;	// this thread runs the next chunk's step 0
+			const u32 hw = a.pwarps[2];			// hand-over: warps of the parse/flush group
+			const bool sg = beside && warp >= hw;	// this thread runs the next chunk's step 0
 			if (step < npass || sg) {
 				// group of this step's loads and insertion: the whole CTA, or the search group
-				const u32 gt = sg ? tid - 32 * LZ_PWARPS : tid, gw = sg ? LZ_WARPS - LZ_PWARPS : LZ_WARPS, gn = 32 * gw;
+				const u32 gt = sg ? tid - 32 * hw : tid, gw = sg ? LZ_WARPS - hw : LZ_WARPS, gn = 32 * gw;
 				auto gbar = [&]() {
-					if (sg) LDB_BAR_SYNC(LZ_BAR_S, LZ_THREADS - 32 * LZ_PWARPS);
+					if (sg) LDB_BAR_SYNC(LZ_BAR_S, LZ_THREADS - 32 * hw);
 					else __syncthreads();
 				};
 				const u8 *src = sg ? (const u8 *)a.in_ptrs[c1] : in;
@@ -1872,13 +1942,20 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					}
 					gbar();
 				}
-				// (b) the group links this pass into the hash chains (ordered within a hash)
+				// (b) the group links this pass into the hash chains (ordered within a hash).  Levels 1-9:
+				// the parse of pass step - 1 comes next, and whether its block ends there depends on the
+				// classes of this pass (counted during the previous step's search), so the block end is
+				// decided here, before the step splits (sized by that decision).
 				LZ_T(0);	// loads + first-pass extras
 				u32 *cmat = sg ? (u32 *)(nextt + 2 * LZ_PASS) : (u32 *)(sm + LZ_SM_R);
+				const bool decide = pipe && !sg && step > LZ_DICT / LZ_PASS;
+				auto decided = [&]() { lz_end_block_decide(v, pass_in_block + 1, b0 - block_begin); };
 #ifdef LZ_TIMING
-				lz_insert_pass_par(ring, head, nextt, cmat, fb0, fpend, fn, gt, lane, warp - (sg ? LZ_PWARPS : 0), gw, gbar, tacc, tlast);
+				lz_insert_pass_par(ring, head, nextt, cmat, fb0, fpend, fn, gt, lane, warp - (sg ? hw : 0), gw, gbar,
+						   decide, decided, tacc, tlast);
 #else
-				lz_insert_pass_par(ring, head, nextt, cmat, fb0, fpend, fn, gt, lane, warp - (sg ? LZ_PWARPS : 0), gw, gbar);
+				lz_insert_pass_par(ring, head, nextt, cmat, fb0, fpend, fn, gt, lane, warp - (sg ? hw : 0), gw, gbar,
+						   decide, decided);
 #endif
 				LZ_T(3);	// insertion: linking
 				if (step == 0) LZ_TSPAN_END(17);
@@ -1903,29 +1980,39 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				LZ_T(1);	// search phase (barrier to barrier)
 				parse_and_flush(b0, pend, pass_in_block * LZ_PASS, nextt + ((b0 + LZ_PASS) & 0xffff));
 			} else {
-				GW = step < npass || beside ? LZ_PWARPS : LZ_WARPS;
+				GW = step < npass ? (v->end_block ? a.pwarps[1] : a.pwarps[0]) : (beside ? hw : LZ_WARPS);
 				GT = 32 * GW;
+				LZ_TSPLIT_BEGIN();
 				if (tid < GT && step > LZ_DICT / LZ_PASS) {
 					const u32 kb0 = b0 - LZ_PASS;
 					parse_and_flush(kb0, kb0 + LZ_PASS < n ? kb0 + LZ_PASS : n, ((step - 1) & 1) * LZ_PASS,
 							nextt + ((kb0 + (beside ? 0 : 2 * LZ_PASS)) & 0xffff));
-					if (beside) {
-						finish();
-						LDB_BAR_SYNC(LZ_BAR_H, LZ_THREADS);	// the next chunk's insert(0) is done
-					}
+					if (beside) finish();
+					LZ_TSPLIT_BUSY();
+					if (beside) LDB_BAR_SYNC(LZ_BAR_H, LZ_THREADS);	// the next chunk's insert(0) is done
 				}
-				if ((step < npass && (!PIECES || step >= v->dict / LZ_PASS)) || beside)
-					search_pass(beside ? 0 : b0, beside ? (n1 < LZ_PASS ? n1 : LZ_PASS) : pend, res + (beside ? 0 : (step & 1) * LZ_PASS),
-						    beside ? n1 : n, beside ? v->nx_min_len : v->min_len, beside ? v->nx_far4 : v->far4_dist);
+				if ((step < npass && (!PIECES || step >= v->dict / LZ_PASS)) || beside) {
+					const u32 spend = beside ? (n1 < LZ_PASS ? n1 : LZ_PASS) : pend, snn = beside ? n1 : n;
+					// the last warps, searchers at every group size, first count the classes of the pass
+					// after this one (loaded already) for the next step's block-end test: the search group
+					// has time to spare at the join, the whole-CTA insertion has none
+					if (warp >= LZ_GROUP_MAX && spend < snn)
+						lz_observe(ring, spend, spend + LZ_PASS < snn ? spend + LZ_PASS : snn, v->obs_next,
+							   tid - 32 * LZ_GROUP_MAX, lane, LZ_THREADS - 32 * LZ_GROUP_MAX);
+					search_pass(beside ? 0 : b0, spend, res + (beside ? 0 : (step & 1) * LZ_PASS), snn,
+						    beside ? v->nx_min_len : v->min_len, beside ? v->nx_far4 : v->far4_dist);
+				}
 				LZ_T(1);	// search (parse/flush group: its share of the search)
 				if (tid == 0) {
 					v->obit_lo = (u32)o.obit; v->obit_hi = (u32)(o.obit >> 32);
 					v->blk_begin = block_begin; v->blk_entry = block_entry; v->blk_passes = pass_in_block;
 				}
-				if (beside && tid == 32 * LZ_PWARPS) v->prefetched = 2;
+				if (beside && tid == LZ_THREADS - 32) v->prefetched = 2;
 			}
+			LZ_TJOIN_BEGIN();
 			__syncthreads();
 			LZ_T(14);	// wait at the join
+			LZ_TSPLIT_END(pipe && step > LZ_DICT / LZ_PASS && (step < npass || beside), beside ? 2 : (v->blk_passes == 0 ? 1 : 0));
 			if (step == npass) LZ_TSPAN_END(16);
 			if (beside) { handed = true; break; }
 			if (v->failed) break;
@@ -1943,28 +2030,40 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		LZ_T(7);	// chunk prologue/epilogue
 	}
 #ifdef LZ_TIMING
-	if (tid == 0 || tid == 32 * LZ_PWARPS)
-		for (int k = 0; k < 18; k++) atomicAdd(&ldb_lz_timing[tid != 0][k], (unsigned long long)tacc[k]);
+	if (LZ_TCLK)
+		for (int k = 0; k < LZ_TSLOTS; k++) atomicAdd(&ldb_lz_timing[tid != 0][k], (unsigned long long)tacc[k]);
 #endif
 }
 
 #ifdef LZ_TIMING
 extern "C" __attribute__((visibility("default"))) void ldb_lz_timing_dump(void)
 {
-	unsigned long long h[2][18], z[2][18] = {};
+	unsigned long long h[2][LZ_TSLOTS], z[2][LZ_TSLOTS] = {};
 	cudaDeviceSynchronize();
 	cudaMemcpyFromSymbol(h, ldb_lz_timing, sizeof(h));
 	cudaMemcpyToSymbol(ldb_lz_timing, z, sizeof(z));
 	const char *names[18] = {"loads+first", "search", "parse e5", "insert: linking", "huffman", "precode", "cost+emit", "chunk pro/epilogue",
 				 "parse e1 steps", "parse e2 walks", "parse e3 exit", "parse e4", "insert: hashing", "insert: slice lists", "wait at join", "",
 				 "(span) last step", "(span) step 0 load+insert"};
-	const char *who[2] = {"thread 0 (parse/flush group; levels 10-12: whole CTA)", "first thread of the search group"};
+	const char *who[2] = {"thread 0 (parse/flush group; levels 10-12: whole CTA)", "first thread of the last warp (search group)"};
 	for (int g = 0; g < 2; g++) {
 		unsigned long long tot = 0;
 		for (int k = 0; k < 15; k++) tot += h[g][k];
 		printf("  timing, clocked by %s:\n", who[g]);
 		for (int k = 0; k < 18; k++)
 			if (h[g][k]) printf("  timing %-26s %14llu cycles  %5.1f%%\n", names[k], h[g][k], 100.0 * (double)h[g][k] / (double)tot);
+	}
+	// split steps by kind, cycles per step: span (split to join), parse/flush group busy, each group's join wait
+	const char *kinds[3] = {"parse only", "parse + flush", "hand-over"};
+	unsigned long long all_span = 0;
+	for (int k = 0; k < 3; k++) all_span += h[1][27 + k];
+	printf("  timing split steps       steps   span/step   p-busy/step  s-wait/step  p-wait/step  s-wait %%span  s-wait %%all-split\n");
+	for (int k = 0; k < 3; k++) {
+		const double ns = h[1][24 + k] ? (double)h[1][24 + k] : 1.0;
+		printf("  timing %-15s %10llu %11.0f %13.0f %12.0f %12.0f %12.1f%% %12.1f%%\n", kinds[k], h[1][24 + k], h[1][27 + k] / ns,
+		       h[0][18 + k] / ns, h[1][21 + k] / ns, h[0][21 + k] / ns,
+		       h[1][27 + k] ? 100.0 * (double)h[1][21 + k] / (double)h[1][27 + k] : 0.0,
+		       all_span ? 100.0 * (double)h[1][21 + k] / (double)all_span : 0.0);
 	}
 }
 #endif
@@ -1983,6 +2082,7 @@ static int ldb_launch_deflate_lz(const ldb_deflate_args &a, const ldb_launch_cfg
 						cudaFuncAttributeMaxDynamicSharedMemorySize, LZ_SM_BYTES));
 	ldb_deflate_args b = a;
 	b.work_counter = (u32 *)a.scratch;
+	ldb_deflate_groups(a.level, b.pwarps);
 	LDB_CUDA_CHECK_RET(cudaMemsetAsync(b.work_counter, 0, sizeof(u32), (cudaStream_t)stream));
 	size_t blocks = a.n < (size_t)ldb_deflate_grid(cfg) ? a.n : (size_t)ldb_deflate_grid(cfg);
 	if (a.piece)

@@ -306,12 +306,16 @@ struct ldb_deflate_args {
 	size_t n;
 	int format;
 	int level;
+	// levels 1-9: warps of the parse/flush group in a step that only parses, one that also flushes a block,
+	// and a chunk's last step beside the next chunk's first (set by the launch: ldb_deflate_groups)
+	u32 pwarps[3];
 };
 #define LDB_PIECE_NONFINAL 0x80000000u
 #define LDB_PIECE_DICT_MASK 0x7fffffffu
 int ldb_launch_deflate(const ldb_deflate_args &a, const ldb_launch_cfg &cfg, void *stream);
 size_t ldb_deflate_scratch_bytes(const ldb_launch_cfg &cfg, size_t n);
 int ldb_deflate_grid(const ldb_launch_cfg &cfg);
+void ldb_deflate_groups(int level, u32 pwarps[3]);
 
 // large_kernels.cu: one buffer -> one stream, cut into pieces of LDB_LARGE_PIECE input bytes (the
 // value of LIBDEFLATE_B200_LARGE_PIECE), processed in waves of consecutive pieces.
