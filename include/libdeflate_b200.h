@@ -244,6 +244,63 @@ libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *ctx, int format,
 				    void *out, size_t out_avail, size_t *out_nbytes);
 
 /*
+ * ONE DEFLATE / zlib / gzip stream written call by call (zlib's deflate() loop), each call compressed by
+ * the whole GPU as compress_large pieces.  For input that arrives over time or does not fit in device
+ * memory at once; a stream keeps only its last 32 KiB of input, the input not compressed yet (at most one
+ * piece) and its running checksum and length in device memory (about 160 KiB), so many streams can live on
+ * one context.  A stream belongs to one context and is destroyed before it.
+ *
+ * write appends in_nbytes of input and writes the bytes this call produces, and only those, to out; the
+ * stream is the concatenation of every call's output in call order.  Pieces are LIBDEFLATE_B200_LARGE_PIECE
+ * input bytes, counted from the stream start or from the last flush:
+ *   NO_FLUSH   a complete piece is compressed once at least one more byte follows it (only then is it
+ *              known not to be final): afterwards 1 ... LIBDEFLATE_B200_LARGE_PIECE bytes stay pending
+ *              (0 if nothing has been written).
+ *   SYNC_FLUSH everything pending is compressed as non-final pieces: the output so far ends byte-aligned
+ *              (an empty stored block 00 00 FF FF, or a complete stored block) and any inflater fed it yields
+ *              exactly the input so far.  A flush with nothing pending writes nothing.
+ *   FINISH     the pending bytes become the final piece, followed by the trailer; the stream is finished
+ *              and every later write returns an error code (last_error() says "finished").
+ * The header comes with the stream's first output.  The trailer's CRC-32 / Adler-32 and length (gzip ISIZE:
+ * the total mod 2^32) are carried on the device from call to call.  Without SYNC_FLUSH the stream is
+ * byte-identical to libdeflate_b200_compress_large(format, level, all input) however the input is cut into
+ * writes, zero-length ones included (a total of at most one piece is compress_batch's stream, as there).
+ * A SYNC_FLUSH at a multiple of the piece size changes no byte when more input follows it.  A piece's
+ * dictionary is min(32 KiB, the stream bytes before it rounded down to 16 KiB): 32 KiB except right after
+ * an early flush.
+ *
+ * compress_stream_create: level in [0,12] (-1 = 6); NULL (last_error() says why) on a bad format or level.
+ * compress_stream_bound: an out_avail that suffices for write(s, in_nbytes, flush); it depends only on the
+ *   host-side state (bytes pending, header written) and in_nbytes.  On a fresh stream
+ *   bound(s, n, FINISH) == libdeflate_b200_compress_large_bound(format, n).
+ * compress_stream_write: device pointers, asynchronous on the context's stream: the input is copied in
+ *   stream order, *d_out_nbytes (device) receives this call's output size.  Returns -1, before anything is
+ *   done (no input consumed, nothing written, the stream unchanged), when out_avail is below the bound;
+ *   with enough room nothing can fail on the device.  Input bytes are processed in waves of at most
+ *   LIBDEFLATE_B200_LARGE_WAVE_KB (default 1 GiB); the output does not depend on it.
+ * compress_stream_write_host: host buffers, synchronous, staging included; *out_nbytes is a host size_t.
+ * Kernel time as for compress_large: setup and stitch as kind 6, deflate as 4, checksums as 0 / 1.
+ */
+#define LIBDEFLATE_B200_NO_FLUSH    0
+#define LIBDEFLATE_B200_SYNC_FLUSH  1
+#define LIBDEFLATE_B200_FINISH      2
+struct libdeflate_b200_compress_stream;
+LIBDEFLATEAPI struct libdeflate_b200_compress_stream *
+libdeflate_b200_compress_stream_create(struct libdeflate_b200_ctx *ctx, int format, int level);
+LIBDEFLATEAPI void
+libdeflate_b200_compress_stream_destroy(struct libdeflate_b200_compress_stream *s);
+LIBDEFLATEAPI size_t
+libdeflate_b200_compress_stream_bound(const struct libdeflate_b200_compress_stream *s, size_t in_nbytes, int flush);
+LIBDEFLATEAPI int
+libdeflate_b200_compress_stream_write(struct libdeflate_b200_compress_stream *s,
+				      const void *d_in, size_t in_nbytes, int flush,
+				      void *d_out, size_t out_avail, size_t *d_out_nbytes);
+LIBDEFLATEAPI int
+libdeflate_b200_compress_stream_write_host(struct libdeflate_b200_compress_stream *s,
+					   const void *in, size_t in_nbytes, int flush,
+					   void *out, size_t out_avail, size_t *out_nbytes);
+
+/*
  * ONE large DEFLATE / zlib / gzip stream -> its bytes, decoded by the whole GPU where the stream carries
  * byte-aligned sync points: non-final empty stored blocks (00 00 FF FF), as written after every piece by
  * libdeflate_b200_compress_large, at every flush by zlib's Z_SYNC_FLUSH / Z_FULL_FLUSH, and between pigz's

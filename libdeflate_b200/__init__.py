@@ -13,6 +13,7 @@ Names follow the reference: ``Compressor`` / ``Decompressor`` wrap
 """
 import ctypes
 import os
+import weakref
 from ctypes import POINTER, c_char_p, c_int, c_int32, c_size_t, c_uint, c_uint32, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -50,8 +51,11 @@ BATCH_SYMBOLS = [
     "libdeflate_b200_bgzf_compress_bound", "libdeflate_b200_bgzf_compress", "libdeflate_b200_bgzf_decompress",
     "libdeflate_b200_compress_large_bound", "libdeflate_b200_compress_large", "libdeflate_b200_compress_large_host",
     "libdeflate_b200_decompress_large", "libdeflate_b200_decompress_large_host", "libdeflate_b200_decompress_large_segments",
+    "libdeflate_b200_compress_stream_create", "libdeflate_b200_compress_stream_destroy", "libdeflate_b200_compress_stream_bound",
+    "libdeflate_b200_compress_stream_write", "libdeflate_b200_compress_stream_write_host",
 ]
 LARGE_PIECE = 131072    # LIBDEFLATE_B200_LARGE_PIECE: input bytes per piece of compress_large
+NO_FLUSH, SYNC_FLUSH, FINISH = 0, 1, 2     # flush modes of a compress stream's write
 
 
 class Options(ctypes.Structure):
@@ -172,6 +176,16 @@ def load_library(path=None):
     lib.libdeflate_b200_decompress_large_host.argtypes = [P, c_int, c_uint, P, S, P, S, PS, PS, POINTER(c_int32)]
     lib.libdeflate_b200_decompress_large_segments.restype = S
     lib.libdeflate_b200_decompress_large_segments.argtypes = [P]
+    lib.libdeflate_b200_compress_stream_create.restype = P
+    lib.libdeflate_b200_compress_stream_create.argtypes = [P, c_int, c_int]
+    lib.libdeflate_b200_compress_stream_destroy.restype = None
+    lib.libdeflate_b200_compress_stream_destroy.argtypes = [P]
+    lib.libdeflate_b200_compress_stream_bound.restype = S
+    lib.libdeflate_b200_compress_stream_bound.argtypes = [P, S, c_int]
+    lib.libdeflate_b200_compress_stream_write.restype = c_int
+    lib.libdeflate_b200_compress_stream_write.argtypes = [P, P, S, c_int, P, S, P]
+    lib.libdeflate_b200_compress_stream_write_host.restype = c_int
+    lib.libdeflate_b200_compress_stream_write_host.argtypes = [P, P, S, c_int, P, S, PS]
     return lib
 
 
@@ -262,12 +276,15 @@ class Context:
         self.l = library or lib()
         self.device = device
         self.h = self.l.libdeflate_b200_ctx_create(device)
+        self._streams = weakref.WeakSet()     # compress streams on this context: destroyed before it
         if not self.h:
             raise Error("libdeflate_b200_ctx_create(%d) failed: %s (no CPU fallback exists)"
                         % (device, self.l.libdeflate_b200_last_error().decode()))
 
     def close(self):
         if self.h:
+            for s in list(self._streams):
+                s.close()
             self.l.libdeflate_b200_ctx_destroy(self.h)
             self.h = None
 
@@ -417,6 +434,10 @@ class Context:
             return res.value, None, 0, 0
         return SUCCESS, ctypes.string_at(out, aout.value), ain.value, aout.value
 
+    def compressobj(self, level=6, fmt=RAW):
+        """A CompressStream on this context: ONE stream written call by call, like zlib.compressobj."""
+        return CompressStream(self, level, fmt)
+
     def large_segments(self):
         """Segments the last decompress_large decoded in parallel (1: one lane)."""
         return self.l.libdeflate_b200_decompress_large_segments(self.h)
@@ -494,6 +515,64 @@ class Context:
         finally:
             for p in (d_data, d_ptrs, d_sizes, d_vals):
                 self.l.libdeflate_b200_device_free(self.h, p)
+
+
+class CompressStream:
+    """libdeflate_b200_compress_stream, shaped like zlib.compressobj: compress(data) -> bytes (NO_FLUSH),
+    flush(mode=FINISH) -> bytes (SYNC_FLUSH or FINISH).  Every call compresses the pieces it completes with
+    the whole GPU; the bytes returned by all calls, in order, are one stream.  Host buffers; each output
+    buffer is sized by compress_stream_bound."""
+
+    def __init__(self, ctx, level=6, fmt=RAW):
+        self.ctx = ctx
+        self.l = ctx.l
+        self.h = self.l.libdeflate_b200_compress_stream_create(ctx.h, fmt, level)
+        if not self.h:
+            raise Error("compress_stream_create(fmt=%d, level=%d) failed: %s"
+                        % (fmt, level, self.l.libdeflate_b200_last_error().decode()))
+        ctx._streams.add(self)
+
+    def bound(self, nbytes, flush=NO_FLUSH):
+        return self.l.libdeflate_b200_compress_stream_bound(self.h, nbytes, flush)
+
+    def write(self, data, flush=NO_FLUSH, out_avail=None):
+        """One write_host call: its output bytes, or None when out_avail was below the bound (nothing done)."""
+        if not self.h:
+            raise Error("compress stream is closed")
+        addr, n, keep = _buf_ptr(data)
+        avail = self.bound(n, flush) if out_avail is None else out_avail
+        out = ctypes.create_string_buffer(max(avail, 1))
+        r = c_size_t(0)
+        rc = self.l.libdeflate_b200_compress_stream_write_host(self.h, addr, n, flush, out, avail, ctypes.byref(r))
+        if rc == -1:
+            return None
+        self.ctx._check(rc, "compress_stream_write_host")
+        return ctypes.string_at(out, r.value)
+
+    def compress(self, data):
+        return self.write(data, NO_FLUSH)
+
+    def flush(self, mode=FINISH):
+        if mode not in (SYNC_FLUSH, FINISH):
+            raise ValueError("flush mode must be SYNC_FLUSH or FINISH")
+        return self.write(b"", mode)
+
+    def close(self):
+        if self.h:
+            self.l.libdeflate_b200_compress_stream_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def crc32(data, crc=0):

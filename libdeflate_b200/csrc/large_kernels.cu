@@ -4,43 +4,49 @@
 // kernel as a raw chunk whose match finder is primed with the 32 KiB of input before it, and every
 // piece but the last ends with an empty stored block, i.e. on a byte boundary with BFINAL = 0
 // (ldb_deflate_args::piece).  The kernels here do the rest, per wave of consecutive pieces:
-//   setup  -- the piece pointer / size / slot arrays of the wave, from (in, n, P) alone;
+//   setup  -- the piece pointer / size / slot / dictionary arrays of the wave, from (in, n, P, the
+//             stream bytes before in) alone;
 //   plan   -- one CTA: exact prefix sums of the piece sizes (the offsets of the pieces in the
-//             stream), the fit check, the running CRC-32 / Adler-32 combined from the per-piece
-//             checksums, the wrapper header (first wave) and trailer (last wave);
+//             call's output), the fit check, the running CRC-32 / Adler-32 combined from the
+//             per-piece checksums, the wrapper header (stream start) and trailer (final piece);
 //   copy   -- one CTA per piece: its bytes from its slot to out + header + offset, any alignment.
 // The running offset, checksum and failure flag live in device memory (ldb_large_state), so the
-// waves are queued without waiting.  Algorithmic HBM bytes of the stitch: the stream read and
+// waves are queued without waiting.  compress_large runs the waves of one call over one buffer; a
+// compress stream (DESIGN.md 4.7) runs them call after call over its staged input, its state kept
+// in the stream's own device buffer.  Algorithmic HBM bytes of the stitch: the stream read and
 // written once.
 #include "ldb_common.cuh"
 
-__device__ __forceinline__ u32 lg_hdr_bytes(int format) { return format == LDB_FMT_GZIP ? 10 : (format == LDB_FMT_ZLIB ? 2 : 0); }
 __device__ __forceinline__ u32 lg_trl_bytes(int format) { return format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0); }
 
 __global__ void __launch_bounds__(256)
 ldb_large_setup_kernel(ldb_large_args a)
 {
 	const size_t gtid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-	if (gtid == 0 && a.first == 0) {
+	if (gtid == 0 && a.call_start) {
 		a.state->offset = 0;
-		a.state->sum_len = 0;
-		a.state->sum = a.format == LDB_FMT_ZLIB ? 1 : 0;
 		a.state->failed = 0;
 	}
+	if (gtid == 0 && a.stream_start) {
+		a.state->sum_len = 0;
+		a.state->sum = a.format == LDB_FMT_ZLIB ? 1 : 0;
+	}
 	for (size_t i = gtid; i < a.count; i += (size_t)gridDim.x * blockDim.x) {
-		const size_t k = a.first + i, off = k * LDB_LARGE_PIECE;
+		const size_t off = i * LDB_LARGE_PIECE;
 		const size_t len = a.in_nbytes - off < LDB_LARGE_PIECE ? a.in_nbytes - off : LDB_LARGE_PIECE;
-		const bool nonfinal = k + 1 < a.npieces;
+		const bool nonfinal = !(a.final_piece && i + 1 == a.count);
+		const u64 before = a.hist + off;	// stream bytes before the piece
+		const u32 dict = before < LDB_LARGE_DICT ? (u32)before & ~(u32)(LDB_LARGE_DICT_STEP - 1) : LDB_LARGE_DICT;
 		a.in_ptrs[i] = a.in + off;
 		a.in_nbytes_k[i] = len;
-		if (a.npieces == 1) {	// the whole input is one ordinary chunk, compressed straight into out
+		if (a.direct) {	// the whole stream is one ordinary chunk, compressed straight into out
 			a.out_ptrs[i] = a.out;
 			a.out_avail_k[i] = a.out_avail;
 			a.piece[i] = 0;
 		} else {
 			a.out_ptrs[i] = a.slots + i * LDB_LARGE_SLOT;
 			a.out_avail_k[i] = ldb_raw_bound(len) + (nonfinal ? 5 : 0);
-			a.piece[i] = (k ? LDB_LARGE_DICT : 0) | (nonfinal ? LDB_PIECE_NONFINAL : 0);
+			a.piece[i] = dict | (nonfinal ? LDB_PIECE_NONFINAL : 0);
 		}
 	}
 }
@@ -107,16 +113,13 @@ ldb_large_plan_kernel(ldb_large_args a)
 		__syncthreads();
 	}
 	if (tid == LG_PLAN_THREADS - 1) {	// (its pos is the end of the wave)
-		const u32 hdr = lg_hdr_bytes(a.format), trl = lg_trl_bytes(a.format);
-		const bool last = a.first + a.count == a.npieces;
+		const u32 hdr = a.hdr, trl = a.final_piece ? lg_trl_bytes(a.format) : 0;
 		const u64 total = pos;
-		const u32 failed = st.failed || any_empty || (u64)hdr + total + (last ? trl : 0) > a.out_avail;
+		const u32 failed = st.failed || any_empty || (u64)hdr + total + trl > a.out_avail;
 		const u32 run = ck ? ldb_sum_combine(a.format, xp, st.sum, tv[0], tl[0]) : 0;
-		if (!failed && a.first == 0) def_write_header(a.out, a.format, a.level);
-		if (last) {
-			if (!failed) def_write_trailer(a.out + hdr + total, a.format, run, a.in_nbytes);
-			*a.out_nbytes = failed ? 0 : (size_t)(hdr + total + trl);
-		}
+		if (!failed && a.stream_start) def_write_header(a.out, a.format, a.level);
+		if (!failed && a.final_piece) def_write_trailer(a.out + hdr + total, a.format, run, st.sum_len + tl[0]);	// (ISIZE: mod 2^32)
+		if (a.call_end) *a.out_nbytes = failed ? 0 : (size_t)(hdr + total + trl);
 		a.state->offset = total;
 		a.state->sum_len = st.sum_len + tl[0];
 		a.state->sum = run;
@@ -144,7 +147,7 @@ __global__ void __launch_bounds__(LG_COPY_THREADS)
 ldb_large_copy_kernel(ldb_large_args a)
 {
 	if (a.state->failed) return;
-	const u32 hdr = lg_hdr_bytes(a.format);
+	const u32 hdr = a.hdr;
 	for (size_t i = blockIdx.x; i < a.count; i += gridDim.x) {
 		const u8 *src = a.slots + i * LDB_LARGE_SLOT;
 		const size_t len = a.out_nbytes_k[i];

@@ -322,35 +322,46 @@ void ldb_deflate_groups(int level, u32 pwarps[3]);
 #ifndef LDB_LARGE_PIECE
 #define LDB_LARGE_PIECE 131072
 #endif
-#define LDB_LARGE_DICT 32768	// input bytes before a piece that prime its match finder
+#define LDB_LARGE_DICT 32768	// input bytes before a piece that prime its match finder (at most)
+#define LDB_LARGE_DICT_STEP 16384	// a dictionary is whole passes of the deflate kernel (LZ_PASS)
 static_assert(LDB_LARGE_PIECE % 16 == 0 && LDB_LARGE_PIECE >= LDB_LARGE_DICT && LDB_LARGE_PIECE <= (1 << 30),
 	      "a piece's dictionary is the input before it");
+static_assert(LDB_LARGE_DICT % LDB_LARGE_DICT_STEP == 0, "the dictionary is whole passes");
 // libdeflate_deflate_compress_bound() (ref: lib/deflate_compress.c:4088-4135)
 __host__ __device__ __forceinline__ size_t ldb_raw_bound(size_t n) { return 5 * (n ? (n + 4999) / 5000 : 1) + n; }
 // device slot of one piece: its bound, the closing empty stored block, and 16 bytes the stitch may read past
 #define LDB_LARGE_SLOT ((ldb_raw_bound(LDB_LARGE_PIECE) + 5 + 15) / 16 * 16 + 16)
-struct ldb_large_state {	// carried from wave to wave on the device
-	u64 offset;		// stream bytes of the pieces stitched so far (after the header)
-	u64 sum_len;		// input bytes the running checksum covers
+struct ldb_large_state {	// carried from wave to wave on the device (and from call to call of a compress stream)
+	u64 offset;		// output bytes of the pieces this call has stitched so far (after its header)
+	u64 sum_len;		// input bytes the running checksum covers: the stream so far
 	u32 sum;		// CRC-32 (gzip) / Adler-32 (zlib) of those bytes
-	u32 failed;		// the stream does not fit (or a piece did not fit its slot)
+	u32 failed;		// this call's output does not fit (or a piece did not fit its slot)
 };
+// One wave: 'count' consecutive pieces of LDB_LARGE_PIECE bytes (the last may be shorter) from 'in' on.
+// The pieces are compressed into the slots and stitched at out + hdr + (the call's output so far).
 struct ldb_large_args {
-	const u8 *in;		// the whole input
-	size_t in_nbytes;
-	u8 *out;		// the stream
+	const u8 *in;		// the wave's first piece; its dictionary, if any, is the input just before it
+	size_t in_nbytes;	// input bytes of the wave's pieces
+	u64 hist;		// stream bytes before 'in' (a piece's dictionary: LDB_LARGE_DICT of them at most,
+				// rounded down to LDB_LARGE_DICT_STEP)
+	u8 *out;		// the call's output
 	size_t out_avail;
-	size_t *out_nbytes;	// device: stream size, or 0 -- written by the last wave
+	size_t *out_nbytes;	// device: the call's output size, or 0 -- written by the call's last wave
 	int format, level;
-	size_t npieces;
-	size_t first, count;	// this wave: pieces [first, first + count)
+	size_t count;
+	u32 hdr;		// wrapper header bytes at the start of the call's output (0: written by an earlier call)
+	u8 direct;		// the wave is one ordinary chunk (the whole stream), compressed with its wrapper into out
+	u8 call_start;		// the call's first wave: the output offset and the failure flag start over
+	u8 stream_start;	// the stream's first wave: the running checksum starts, the header is written
+	u8 call_end;		// the call's last wave: *out_nbytes is written
+	u8 final_piece;		// the wave's last piece ends the stream: it is final, the trailer follows it
 	// per piece of the wave
 	const void **in_ptrs;
 	size_t *in_nbytes_k, *out_avail_k, *out_nbytes_k;
 	void **out_ptrs;
 	u32 *piece, *sums;
 	u64 *offsets;
-	u8 *slots;		// piece first + i is compressed into slots + i * LDB_LARGE_SLOT (16-byte aligned)
+	u8 *slots;		// piece i of the wave is compressed into slots + i * LDB_LARGE_SLOT (16-byte aligned)
 	ldb_large_state *state;
 };
 int ldb_launch_large_setup(const ldb_large_args &a, void *stream);

@@ -104,7 +104,8 @@ struct libdeflate_b200_ctx {
 	ldb_buf tmp;			// device: per-batch u32/size_t arrays
 	ldb_buf d_stage_in, d_stage_out;// device staging for host-buffer calls
 	ldb_buf d_pack;			// device: packed output of the *_packed host calls
-	ldb_buf large;			// device: per-wave piece arrays, state and slots of compress_large
+	ldb_buf large;			// device: per-wave piece arrays, state and slots of compress_large and the compress streams
+	ldb_buf cs_stage;		// device: one wave of a compress stream's input, behind its history
 	// decompress_large (device): sync-point scan + split list, per-wave arrays, re-decoded tokens,
 	// symbol planes, windows, the carried window, the high-plane literal stream, checksum arrays
 	ldb_buf li_scan, li_arr, li_tok2, li_planes, li_win, li_carry, li_hilit, li_sums;
@@ -233,6 +234,7 @@ extern "C" void libdeflate_b200_ctx_destroy(struct libdeflate_b200_ctx *ctx)
 	cudaFree(ctx->d_stage_out.p);
 	cudaFree(ctx->d_pack.p);
 	cudaFree(ctx->large.p);
+	cudaFree(ctx->cs_stage.p);
 	for (ldb_buf *b : {&ctx->li_scan, &ctx->li_arr, &ctx->li_tok2, &ctx->li_planes, &ctx->li_win, &ctx->li_carry, &ctx->li_hilit, &ctx->li_sums})
 		cudaFree(b->p);
 	cudaFree(ctx->d_params.p);
@@ -1075,55 +1077,48 @@ extern "C" size_t libdeflate_b200_compress_large_bound(int format, size_t in_nby
 	return wrap_bytes(format) + full * (ldb_raw_bound(LDB_LARGE_PIECE) + 5) + ldb_raw_bound(in_nbytes - full * LDB_LARGE_PIECE);
 }
 
-extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, int format, int level,
-					       const void *d_in, size_t in_nbytes,
-					       void *d_out, size_t out_avail, size_t *d_out_nbytes)
+// Pieces per wave (default 1 GiB of input; LIBDEFLATE_B200_LARGE_WAVE_KB overrides): the context keeps the
+// compressed slots of one wave, not of the whole input.  No stream depends on it.
+static size_t large_wave_pieces(void)
 {
-	int rc = check_format(format);
-	if (!rc) rc = check_level(&level);
-	if (rc) return rc;
-	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
-	const size_t npieces = in_nbytes ? (in_nbytes + LDB_LARGE_PIECE - 1) / LDB_LARGE_PIECE : 1;
-	// Input bytes per wave (default 1 GiB; LIBDEFLATE_B200_LARGE_WAVE_KB overrides): the context keeps the
-	// compressed slots of one wave, not of the whole input.  The stream does not depend on it.
-	const size_t wave_pieces = std::max((ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_KB", (size_t)1 << 20) << 10) / LDB_LARGE_PIECE, (size_t)1);
-	const size_t wave = npieces < wave_pieces ? npieces : wave_pieces;
-	// ctx->large: in_ptrs | in_nbytes | out_ptrs | out_avail | out_nbytes | offsets | piece | sums | state | slots
+	return std::max((ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_KB", (size_t)1 << 20) << 10) / LDB_LARGE_PIECE, (size_t)1);
+}
+
+static u32 hdr_bytes(int format) { return format == LDB_FMT_GZIP ? 10 : (format == LDB_FMT_ZLIB ? 2 : 0); }
+
+// The context's per-wave room for waves of up to 'wave' pieces -- ctx->large: in_ptrs | in_nbytes | out_ptrs |
+// out_avail | out_nbytes | offsets | piece | sums | state | slots, and the deflate scratch (slots = false: one
+// direct chunk, which compress_batch gives its own) -- laid out in g.  g.state is the context's.
+static int large_layout(libdeflate_b200_ctx *ctx, size_t wave, bool slots, ldb_large_args *g)
+{
 	const size_t a8 = align_up(wave * 8, 256), a4 = align_up(wave * 4, 256);
 	const size_t slots_off = 6 * a8 + 2 * a4 + 256;
-	rc = ldb_reserve_dev(ctx->large, slots_off + (npieces > 1 ? wave * LDB_LARGE_SLOT : 0));
+	int rc = ldb_reserve_dev(ctx->large, slots_off + (slots ? wave * LDB_LARGE_SLOT : 0));
+	if (!rc && slots) rc = ldb_reserve_dev(ctx->deflate_scratch, ldb_deflate_scratch_bytes(ctx->cfg, wave));
 	if (rc) return rc;
 	u8 *b = (u8 *)ctx->large.p;
-	ldb_large_args g;
-	g.in = (const u8 *)d_in;
-	g.in_nbytes = in_nbytes;
-	g.out = (u8 *)d_out;
-	g.out_avail = out_avail;
-	g.out_nbytes = d_out_nbytes;
-	g.format = format;
-	g.level = level;
-	g.npieces = npieces;
-	g.in_ptrs = (const void **)b;
-	g.in_nbytes_k = (size_t *)(b + a8);
-	g.out_ptrs = (void **)(b + 2 * a8);
-	g.out_avail_k = (size_t *)(b + 3 * a8);
-	g.out_nbytes_k = (size_t *)(b + 4 * a8);
-	g.offsets = (u64 *)(b + 5 * a8);
-	g.piece = (u32 *)(b + 6 * a8);
-	g.sums = (u32 *)(b + 6 * a8 + a4);
-	g.state = (ldb_large_state *)(b + 6 * a8 + 2 * a4);
-	g.slots = b + slots_off;
-	if (npieces == 1) {
-		// the whole input is one chunk: exactly what compress_batch makes of it, straight into d_out
-		g.first = 0;
-		g.count = 1;
-		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_setup(g, ctx->stream); });
-		if (rc) return rc;
-		return libdeflate_b200_compress_batch(ctx, format, level, (const void *const *)g.in_ptrs, g.in_nbytes_k,
-						      (void *const *)g.out_ptrs, g.out_avail_k, d_out_nbytes, 1);
-	}
-	rc = ldb_reserve_dev(ctx->deflate_scratch, ldb_deflate_scratch_bytes(ctx->cfg, wave));
+	g->in_ptrs = (const void **)b;
+	g->in_nbytes_k = (size_t *)(b + a8);
+	g->out_ptrs = (void **)(b + 2 * a8);
+	g->out_avail_k = (size_t *)(b + 3 * a8);
+	g->out_nbytes_k = (size_t *)(b + 4 * a8);
+	g->offsets = (u64 *)(b + 5 * a8);
+	g->piece = (u32 *)(b + 6 * a8);
+	g->sums = (u32 *)(b + 6 * a8 + a4);
+	g->state = (ldb_large_state *)(b + 6 * a8 + 2 * a4);
+	g->slots = b + slots_off;
+	return 0;
+}
+
+// One wave: piece setup, per-piece checksums, deflate of the pieces into their slots, stitch.  A direct
+// wave is exactly what compress_batch makes of its one chunk, straight into g.out.
+static int large_wave(libdeflate_b200_ctx *ctx, const ldb_large_args &g)
+{
+	int rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_setup(g, ctx->stream); });
 	if (rc) return rc;
+	if (g.direct)
+		return libdeflate_b200_compress_batch(ctx, g.format, g.level, (const void *const *)g.in_ptrs, g.in_nbytes_k,
+						      (void *const *)g.out_ptrs, g.out_avail_k, g.out_nbytes, 1);
 	ldb_deflate_args a;
 	a.in_ptrs = (const void *const *)g.in_ptrs;
 	a.in_nbytes = g.in_nbytes_k;
@@ -1134,20 +1129,46 @@ extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, i
 	a.scratch = (u8 *)ctx->deflate_scratch.p;
 	a.work_counter = nullptr;
 	a.piece = g.piece;
+	a.n = g.count;
 	a.format = LDB_FMT_RAW;
-	a.level = level;
+	a.level = g.level;
+	rc = launch_checksum(ctx, g.format, a.in_ptrs, a.in_nbytes, g.sums, g.count);
+	if (rc) return rc;
+	rc = ldb_timed_launch(ctx, LDB_K_DEFLATE, [&] { return ldb_launch_deflate(a, ctx->cfg, ctx->stream); });
+	if (rc) return rc;
+	ctx->launches++;	// plan + copy
+	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_stitch(g, ctx->stream); });
+}
+
+extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, int format, int level,
+					       const void *d_in, size_t in_nbytes,
+					       void *d_out, size_t out_avail, size_t *d_out_nbytes)
+{
+	int rc = check_format(format);
+	if (!rc) rc = check_level(&level);
+	if (rc) return rc;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	const size_t npieces = in_nbytes ? (in_nbytes + LDB_LARGE_PIECE - 1) / LDB_LARGE_PIECE : 1;
+	const size_t wave = std::min(npieces, large_wave_pieces());
+	ldb_large_args g;
+	rc = large_layout(ctx, wave, npieces > 1, &g);
+	if (rc) return rc;
+	g.out = (u8 *)d_out;
+	g.out_avail = out_avail;
+	g.out_nbytes = d_out_nbytes;
+	g.format = format;
+	g.level = level;
+	g.hdr = hdr_bytes(format);
+	g.direct = npieces == 1;	// the whole input is one chunk
 	for (size_t first = 0; first < npieces; first += wave) {
-		g.first = first;
-		g.count = npieces - first < wave ? npieces - first : wave;
-		a.n = g.count;
-		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_setup(g, ctx->stream); });
-		if (rc) return rc;
-		rc = launch_checksum(ctx, format, a.in_ptrs, a.in_nbytes, g.sums, g.count);
-		if (rc) return rc;
-		rc = ldb_timed_launch(ctx, LDB_K_DEFLATE, [&] { return ldb_launch_deflate(a, ctx->cfg, ctx->stream); });
-		if (rc) return rc;
-		ctx->launches++;	// plan + copy
-		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_stitch(g, ctx->stream); });
+		const size_t off = first * LDB_LARGE_PIECE;
+		g.in = (const u8 *)d_in + off;
+		g.hist = off;
+		g.count = std::min(wave, npieces - first);
+		g.in_nbytes = std::min(g.count * LDB_LARGE_PIECE, in_nbytes - off);
+		g.call_start = g.stream_start = first == 0;
+		g.call_end = g.final_piece = first + g.count == npieces;
+		rc = large_wave(ctx, g);
 		if (rc) return rc;
 	}
 	return 0;
@@ -1173,6 +1194,211 @@ extern "C" int libdeflate_b200_compress_large_host(struct libdeflate_b200_ctx *c
 	if (!rc) rc = read_back(ctx, out, ctx->d_stage_out.p, r);
 	if (rc) return rc;
 	*out_nbytes = r;
+	return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// one stream, written call by call (DESIGN.md 4.7): the compress_large waves over staged input
+// ---------------------------------------------------------------------------------
+// The stream's device buffer: [history: the last <= 32 KiB of input before the pending bytes, right-aligned
+// at CS_PEND | pending: at most one piece | ldb_large_state].  The staging area of a call (ctx->cs_stage) has the
+// same front: [history | the wave's pieces], so the first piece of every wave starts 16-byte aligned.
+#define CS_PEND LDB_LARGE_DICT
+#define CS_STATE (LDB_LARGE_DICT + LDB_LARGE_PIECE)
+#define CS_BUF_BYTES (CS_STATE + 256)
+
+struct libdeflate_b200_compress_stream {
+	libdeflate_b200_ctx *ctx;
+	int format, level;
+	u8 *d_buf;
+	size_t pending;		// input bytes not compressed yet
+	size_t hist;		// bytes of history before them: min(32 KiB, the stream bytes before them)
+	u64 total;		// input bytes written so far
+	bool started;		// the header has been written (the stream has produced output)
+	bool finished;
+};
+
+// What one write of n bytes with 'flush' does, from the host-side state alone.
+struct cs_plan {
+	size_t emit;		// bytes compressed: the pending ones first, then the call's
+	size_t pieces;		// pieces they make (a FINISH on nothing pending: one empty final piece)
+	bool direct;		// FINISH of a stream that never produced output, at most one piece: compress_batch
+	bool fin;
+	size_t bound;		// output bytes that always suffice
+};
+
+static cs_plan cs_plan_of(const libdeflate_b200_compress_stream *s, size_t n, int flush)
+{
+	const size_t P = LDB_LARGE_PIECE, t = s->pending + n;
+	cs_plan p{};
+	p.fin = flush == LIBDEFLATE_B200_FINISH;
+	if (p.fin && !s->started && t <= P) {	// compress_large's one-chunk case
+		p.emit = t;
+		p.pieces = 1;
+		p.direct = true;
+		p.bound = wrap_bytes(s->format) + ldb_raw_bound(t);
+		return p;
+	}
+	// without a flush a complete piece waits for one more byte: only then is it known not to be final
+	p.emit = flush == LIBDEFLATE_B200_NO_FLUSH ? (t ? (t - 1) / P * P : 0) : t;
+	p.pieces = (p.emit + P - 1) / P;
+	if (p.fin && !p.pieces) p.pieces = 1;
+	if (!p.pieces) return p;
+	// every piece fits its raw bound; the non-final ones add their closing empty stored block
+	const size_t last = p.emit - (p.pieces - 1) * P;
+	p.bound = (p.pieces - 1) * (ldb_raw_bound(P) + 5) + ldb_raw_bound(last) + (p.fin ? 0 : 5);
+	if (!s->started) p.bound += hdr_bytes(s->format);
+	if (p.fin) p.bound += wrap_bytes(s->format) - hdr_bytes(s->format);
+	return p;
+}
+
+extern "C" struct libdeflate_b200_compress_stream *
+libdeflate_b200_compress_stream_create(struct libdeflate_b200_ctx *ctx, int format, int level)
+{
+	if (!ctx) {
+		ldb_fail(cudaErrorInvalidValue, "compress_stream_create: no context", __FILE__, __LINE__);
+		return nullptr;
+	}
+	if (check_format(format) || check_level(&level)) return nullptr;
+	if (cudaSetDevice(ctx->device) != cudaSuccess) {
+		ldb_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+		return nullptr;
+	}
+	u8 *d = nullptr;
+	if (cudaMalloc((void **)&d, CS_BUF_BYTES) != cudaSuccess) {
+		ldb_fail(cudaGetLastError(), "cudaMalloc(compress stream)", __FILE__, __LINE__);
+		return nullptr;
+	}
+	libdeflate_b200_compress_stream *s = new libdeflate_b200_compress_stream();
+	s->ctx = ctx;
+	s->format = format;
+	s->level = level;
+	s->d_buf = d;
+	s->pending = s->hist = 0;
+	s->total = 0;
+	s->started = s->finished = false;
+	return s;
+}
+
+extern "C" void libdeflate_b200_compress_stream_destroy(struct libdeflate_b200_compress_stream *s)
+{
+	if (!s) return;
+	cudaSetDevice(s->ctx->device);
+	cudaStreamSynchronize(s->ctx->stream);	// (queued writes may still read the buffer)
+	cudaFree(s->d_buf);
+	delete s;
+}
+
+extern "C" size_t libdeflate_b200_compress_stream_bound(const struct libdeflate_b200_compress_stream *s, size_t in_nbytes, int flush)
+{
+	return s && !s->finished ? cs_plan_of(s, in_nbytes, flush).bound : 0;
+}
+
+// The device and host forms: 'in' is read with copies of kind 'in_kind' in stream order, the output goes to
+// d_out, the size to *d_out_nbytes (device); -1 before anything is done when out_avail is below the bound.
+static int cs_write(libdeflate_b200_compress_stream *s, const void *in, size_t n, cudaMemcpyKind in_kind, int flush,
+		    void *d_out, size_t out_avail, size_t *d_out_nbytes)
+{
+	if (!s) return ldb_fail(cudaErrorInvalidValue, "compress_stream_write: no stream", __FILE__, __LINE__);
+	if (s->finished) return ldb_fail(cudaErrorInvalidValue, "compress_stream_write: the stream is finished", __FILE__, __LINE__);
+	if (flush < LIBDEFLATE_B200_NO_FLUSH || flush > LIBDEFLATE_B200_FINISH)
+		return ldb_fail(cudaErrorInvalidValue, "compress_stream_write: flush", __FILE__, __LINE__);
+	if (n && !in) return ldb_fail(cudaErrorInvalidValue, "compress_stream_write: no input", __FILE__, __LINE__);
+	const cs_plan p = cs_plan_of(s, n, flush);
+	if (out_avail < p.bound) return -1;
+	libdeflate_b200_ctx *ctx = s->ctx;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	const u8 *src = (const u8 *)in;
+	u8 *pend = s->d_buf + CS_PEND;
+	if (!p.pieces) {	// the input only joins the pending bytes
+		if (n) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(pend + s->pending, src, n, in_kind, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaMemsetAsync(d_out_nbytes, 0, sizeof(size_t), ctx->stream));
+		s->pending += n;
+		s->total += n;
+		return 0;
+	}
+	const size_t P = LDB_LARGE_PIECE, wave = std::min(p.pieces, large_wave_pieces());
+	ldb_large_args g;
+	int rc = large_layout(ctx, wave, !p.direct, &g);
+	if (!rc) rc = ldb_reserve_dev(ctx->cs_stage, CS_PEND + wave * P + 64);
+	if (rc) return rc;
+	u8 *base = (u8 *)ctx->cs_stage.p + CS_PEND;	// the wave's first piece
+	g.state = (ldb_large_state *)(s->d_buf + CS_STATE);
+	g.out = (u8 *)d_out;
+	g.out_avail = out_avail;
+	g.out_nbytes = d_out_nbytes;
+	g.format = s->format;
+	g.level = s->level;
+	g.hdr = s->started ? 0 : hdr_bytes(s->format);
+	g.direct = p.direct;
+	const u64 before = s->total - s->pending;	// stream bytes before the call's first piece
+	size_t used = 0, hist = s->hist, bytes = 0;	// input bytes staged; history and piece bytes of the wave
+	for (size_t first = 0; first < p.pieces; first += wave) {
+		g.count = std::min(wave, p.pieces - first);
+		bytes = std::min(g.count * P, p.emit - first * P);
+		size_t fresh = bytes;
+		if (first == 0) {	// the stream's history and pending bytes, then the call's input
+			if (s->hist + s->pending)
+				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(base - s->hist, pend - s->hist, s->hist + s->pending, cudaMemcpyDeviceToDevice, ctx->stream));
+			fresh = bytes - s->pending;
+		} else {		// the last 32 KiB of the wave before (wave * P >= 32 KiB bytes: no overlap), then the input
+			hist = LDB_LARGE_DICT;
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(base - hist, base + wave * P - hist, hist, cudaMemcpyDeviceToDevice, ctx->stream));
+		}
+		if (fresh) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(base + (bytes - fresh), src + used, fresh, in_kind, ctx->stream));
+		used += fresh;
+		g.in = base;
+		g.in_nbytes = bytes;
+		g.hist = before + first * P;
+		g.call_start = first == 0;
+		g.stream_start = first == 0 && !s->started;
+		g.call_end = first + g.count == p.pieces;
+		g.final_piece = g.call_end && p.fin;
+		rc = large_wave(ctx, g);
+		if (rc) return rc;
+	}
+	s->total += n;
+	s->started = true;
+	if (p.fin) {
+		s->finished = true;
+		return 0;
+	}
+	// the carry: the last <= 32 KiB compressed, and the input after them (at most one piece)
+	const size_t keep = std::min((size_t)LDB_LARGE_DICT, hist + bytes);
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(pend - keep, base + bytes - keep, keep, cudaMemcpyDeviceToDevice, ctx->stream));
+	if (n > used) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(pend, src + used, n - used, in_kind, ctx->stream));
+	s->hist = keep;
+	s->pending = n - used;
+	return 0;
+}
+
+extern "C" int libdeflate_b200_compress_stream_write(struct libdeflate_b200_compress_stream *s, const void *d_in, size_t in_nbytes,
+						      int flush, void *d_out, size_t out_avail, size_t *d_out_nbytes)
+{
+	return cs_write(s, d_in, in_nbytes, cudaMemcpyDeviceToDevice, flush, d_out, out_avail, d_out_nbytes);
+}
+
+extern "C" int libdeflate_b200_compress_stream_write_host(struct libdeflate_b200_compress_stream *s, const void *in, size_t in_nbytes,
+							   int flush, void *out, size_t out_avail, size_t *out_nbytes)
+{
+	if (out_nbytes) *out_nbytes = 0;
+	if (!s) return ldb_fail(cudaErrorInvalidValue, "compress_stream_write_host: no stream", __FILE__, __LINE__);
+	libdeflate_b200_ctx *ctx = s->ctx;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	stream_quiesce quiesce(ctx);
+	const size_t bound = s->finished ? 0 : cs_plan_of(s, in_nbytes, flush).bound;
+	int rc = ldb_reserve_dev(ctx->d_stage_out, bound + 64);
+	if (!rc) rc = ldb_reserve_dev(ctx->d_params, 256);
+	if (rc) return rc;
+	size_t *d_res = (size_t *)ctx->d_params.p;
+	// (the device sees out_avail = the bound: enough, and the staging stays the size of the output)
+	rc = cs_write(s, in, in_nbytes, cudaMemcpyHostToDevice, flush, ctx->d_stage_out.p, std::min(out_avail, bound), d_res);
+	if (rc) return rc;
+	size_t r = 0;
+	rc = read_back(ctx, &r, d_res, sizeof(r));
+	if (!rc) rc = read_back(ctx, out, ctx->d_stage_out.p, r);
+	if (rc) return rc;
+	if (out_nbytes) *out_nbytes = r;
 	return 0;
 }
 
