@@ -6,10 +6,9 @@
 // lib/gzip_compress.c:32-80, lib/zlib_compress.c:32-72).  Compressed bytes are not
 // contractual (libdeflate.h:76-83) and are NOT the reference's bytes.
 //
-// This file: the stored-block path (wrapper header/trailer writers: ldb_common.cuh)
-// (level 0 and inputs <= 55 - 4*level bytes: ref deflate_compress_none,
-// lib/deflate_compress.c:2393-2443).  The LZ77 + Huffman path is in
-// deflate_lz_kernel.cuh.
+// This file: the level-0 kernel, stored blocks only (def_write_stored_chunk in ldb_common.cuh,
+// which the LZ kernel also uses for inputs <= 55 - 4*level bytes).  The LZ77 + Huffman path is
+// in deflate_lz_kernel.cuh, its block encoder in deflate_block.cuh.
 #include <stdlib.h>
 #include <string.h>
 
@@ -21,41 +20,7 @@
 __global__ void __launch_bounds__(DEF_THREADS)
 ldb_deflate_stored_kernel(ldb_deflate_args a)
 {
-	for (size_t c = blockIdx.x; c < a.n; c += gridDim.x) {
-		const u8 *in = (const u8 *)a.in_ptrs[c];
-		const size_t n = a.in_nbytes[c];
-		u8 *out = (u8 *)a.out_ptrs[c];
-		const size_t avail = a.out_avail[c];
-		const u32 overhead = a.format == LDB_FMT_GZIP ? 18 : (a.format == LDB_FMT_ZLIB ? 6 : 0);
-		const u32 hdr = a.format == LDB_FMT_GZIP ? 10 : (a.format == LDB_FMT_ZLIB ? 2 : 0);
-		const size_t nblocks = n ? (n + 65534) / 65535 : 1;
-		const size_t need = n + 5 * nblocks;
-		// the wrappers refuse avail <= overhead outright (gzip_compress.c:40, zlib_compress.c:42)
-		bool fits = !(overhead && avail <= overhead) && need <= avail - overhead;
-		if (!fits) {
-			if (threadIdx.x == 0) a.out_nbytes[c] = 0;
-			continue;
-		}
-		if (threadIdx.x == 0) def_write_header(out, a.format, a.level);
-		// a non-final piece of a larger stream: stored blocks end byte-aligned, so no BFINAL is all it needs
-		const bool final_piece = !(a.piece && (a.piece[c] & LDB_PIECE_NONFINAL));
-		u8 *dst = out + hdr;
-		for (size_t b = 0; b < nblocks; b++) {
-			size_t off = b * 65535;
-			u32 len = (u32)(n - off > 65535 ? 65535 : n - off);
-			if (threadIdx.x == 0) {
-				dst[0] = (b + 1 == nblocks && final_piece) ? 1 : 0;	// BFINAL, BTYPE = 00
-				dst[1] = (u8)len; dst[2] = (u8)(len >> 8);
-				dst[3] = (u8)~len; dst[4] = (u8)(~len >> 8);
-			}
-			for (u32 i = threadIdx.x; i < len; i += DEF_THREADS) dst[5 + i] = in[off + i];
-			dst += 5 + len;
-		}
-		if (threadIdx.x == 0) {
-			u32 t = def_write_trailer(dst, a.format, a.checksums ? a.checksums[c] : 0, n);
-			a.out_nbytes[c] = (size_t)(dst - out) + t;
-		}
-	}
+	for (size_t c = blockIdx.x; c < a.n; c += gridDim.x) def_write_stored_chunk(a, c, threadIdx.x, DEF_THREADS);
 }
 
 #include "deflate_lz_kernel.cuh"

@@ -1,5 +1,5 @@
 // deflate_lz_kernel.cuh -- LZ77 match finding + parsing + Huffman block encoding, sm_90a.
-// Included by deflate_kernel.cu.
+// Included by deflate_kernel.cu; the block encoder is deflate_block.cuh.
 //
 // Reference behaviour covered (what, not how):
 //   hash-chain match finder            lib/hc_matchfinder.h:182-399, lib/matchfinder_common.h:168-222
@@ -30,12 +30,11 @@
 //         a prefix sum places the tokens,
 //   * tokens and per-position results go to a per-CTA buffer in global memory (L2
 //     resident), symbol histograms stay in shared memory,
-//   * per block (32 KiB of input): Huffman codes (length-limited to 15; parallel except
-//     for the two-queue merge), exact bit cost of dynamic / static / stored (the
-//     reference's three-way choice, which is also what makes
-//     libdeflate_*_compress_bound() hold), then a two-pass emission: per-token bit
-//     lengths -> block-wide exclusive prefix sum -> every thread ORs its codewords
-//     into a shared-memory staging buffer -> coalesced stores,
+//   * per block (32 KiB of input), by the block encoder (deflate_block.cuh): Huffman codes
+//     length-limited to 15, exact bit cost of dynamic / static / stored (the reference's
+//     three-way choice, which is also what makes libdeflate_*_compress_bound() hold), then a
+//     two-pass emission: per-token bit lengths -> group-wide exclusive prefix sum -> every
+//     thread ORs its codewords into a shared-memory staging buffer -> coalesced stores,
 //   * levels 10-12: all matches per position + iterated min-cost-path DP (see below).
 //
 // Algorithmic HBM bytes per chunk: in_nbytes (read once) + out_nbytes (written once).
@@ -148,7 +147,7 @@ struct lz_vars {
 	u32 chunk;
 	u32 tok_count;		// tokens in the current block
 	u32 parse_entry;	// absolute position where the parser continues
-	u32 cost_dyn, cost_static, extra_bits;
+	u32 cost_dyn, cost_static;
 	u32 hlit, hdist, hclen;
 	u32 n_items;
 	u32 run_counter;	// next unassigned search run of the current pass
@@ -287,89 +286,7 @@ __device__ __forceinline__ u32 lz_off_slot(u32 off)	// off 1..32768 -> 0..29
 __device__ __forceinline__ u32 lz_off_extra_bits(u32 slot) { return slot < 4 ? 0 : (slot - 2) >> 1; }
 __device__ __forceinline__ u32 lz_off_base(u32 slot) { return slot < 4 ? 1 + slot : 1 + ((2 + (slot & 1)) << ((slot - 2) >> 1)); }
 
-__device__ __forceinline__ u32 lz_static_litlen_len(u32 sym) { return sym < 144 ? 8 : (sym < 256 ? 9 : (sym < 280 ? 7 : 8)); }
-
-// ---- output bit staging ----------------------------------------------------------------
-// The stream is assembled in 32-bit words relative to the START of the chunk's output
-// buffer.  stage[0] is the word containing bit position 'obit' rounded down.
-struct lz_out {
-	u8 *out;
-	size_t avail;
-	u64 obit;		// bits emitted so far (from the start of 'out', wrapper header included)
-};
-
-__device__ __forceinline__ void lz_stage_or(u32 *stage, u32 rel_bit, u64 bits, u32 nbits)
-{
-	if (!nbits) return;
-	u32 w = rel_bit >> 5, sh = rel_bit & 31;
-	atomicOr(&stage[w], (u32)(bits << sh));
-	if (sh + nbits > 32) {
-		u64 rest = bits >> (32 - sh);
-		atomicOr(&stage[w + 1], (u32)rest);
-		if (sh + nbits > 64) atomicOr(&stage[w + 2], (u32)(rest >> 32));
-	}
-}
-
-// Writes staging words [0, nwords) to the output at word index 'first_word'; threads [0, nthreads).
-__device__ __forceinline__ void lz_flush_words(const lz_out &o, const u32 *stage, u64 first_word, u32 nwords, u32 nthreads)
-{
-	if ((((uintptr_t)o.out) & 3) == 0) {
-		u32 *dst = (u32 *)o.out + first_word;
-		for (u32 i = threadIdx.x; i < nwords; i += nthreads) dst[i] = stage[i];
-	} else {
-		u8 *dst = o.out + first_word * 4;
-		for (u32 i = threadIdx.x; i < nwords * 4; i += nthreads) dst[i] = (u8)(stage[i >> 2] >> (8 * (i & 3)));
-	}
-}
-
-// ---- Huffman code construction ---------------------------------------------------------
-// (ref for the length-limiting idea: deflate_compress.c:1023-1091; at least two codewords like
-// deflate_compress.c:1369-1378; the parallel parts live in the kernel's build_codes step)
-// Two-queue Huffman merge only (one thread): leaves nodefreq[0, nused) ascending, internal nodes
-// appended behind them; writes parent[] for every node but the root.  The two queue heads and their
-// successors are kept in registers so that a shared-memory load is never waited for directly.
-__device__ __forceinline__ void lz_huffman_merge(u32 *nodefreq, u16 *parent, u32 nused)
-{
-	const u32 INF = 0xffffffffu;
-	u32 leaf = 0, inode = nused, nn = nused;
-	u32 l0 = nodefreq[0], l1 = nused > 1 ? nodefreq[1] : INF;	// leaf queue: head, next
-	u32 n0 = INF, n1 = INF;						// internal queue: head, next
-	while (nn < 2 * nused - 1) {
-		u32 a, b, fa, fb;
-		if (l0 <= n0) { a = leaf++; fa = l0; l0 = l1; l1 = leaf + 1 < nused ? nodefreq[leaf + 1] : INF; }
-		else { a = inode++; fa = n0; n0 = n1; n1 = INF; }
-		if (n0 == INF && inode < nn) n0 = nodefreq[inode];
-		if (l0 <= n0) { b = leaf++; fb = l0; l0 = l1; l1 = leaf + 1 < nused ? nodefreq[leaf + 1] : INF; }
-		else { b = inode++; fb = n0; n0 = n1; n1 = INF; }
-		const u32 sum = fa + fb;
-		nodefreq[nn] = sum;
-		parent[a] = (u16)nn;
-		parent[b] = (u16)nn;
-		nn++;
-		// refill the register copies of the internal queue (the new node may be its head)
-		if (n0 == INF && inode < nn) n0 = inode == nn - 1 ? sum : nodefreq[inode];
-		if (n1 == INF && inode + 1 < nn) n1 = inode + 1 == nn - 1 ? sum : nodefreq[inode + 1];
-	}
-}
-
-// canonical, bit-reversed codewords for an alphabet (all threads participate on disjoint syms)
-__device__ __forceinline__ void lz_gen_codes_serial(const u8 *lens, u32 nsyms, u16 *codes)
-{
-	u32 cnt[16];
-	for (u32 l = 0; l < 16; l++) cnt[l] = 0;
-	for (u32 s = 0; s < nsyms; s++) cnt[lens[s]]++;
-	u32 next[16];
-	u32 code = 0;
-	cnt[0] = 0;
-	for (u32 l = 1; l < 16; l++) {
-		next[l] = code;
-		code = (code + cnt[l]) << 1;
-	}
-	for (u32 s = 0; s < nsyms; s++) {
-		u32 l = lens[s];
-		codes[s] = l ? (u16)(__brev(next[l]++) >> (32 - l)) : 0;
-	}
-}
+#include "deflate_block.cuh"
 
 #ifdef LZ_TIMING
 #include <stdio.h>
@@ -775,6 +692,14 @@ __device__ __forceinline__ void lz_end_block_decide(lz_vars *v, u32 passes, u32 
 	}
 }
 
+// A chunk written as stored blocks (def_write_stored_chunk): tiny (ref: deflate_compress.c:4041-4043),
+// too large for 32-bit positions, or an output buffer the wrapper refuses outright.
+__device__ __forceinline__ bool lz_stored_chunk(size_t n, size_t avail, int format, int level)
+{
+	const u32 overhead = ldb_wrap_bytes(format);
+	return n <= (size_t)(55 - 4 * level) || n > 0x7fff0000u || (overhead && avail <= overhead);
+}
+
 // ---- the kernel ----------------------------------------------------------------------------
 // PIECES: the launch carries ldb_deflate_args::piece (pieces of one stream).  The batch path is the
 // instance without it, where the dictionary is 0 and every chunk final at compile time.
@@ -791,21 +716,11 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 	u32 *vis = (u32 *)(sm + LZ_SM_VIS);
 	u32 *tokoff = (u32 *)(sm + LZ_SM_TOKOFF);
 	u8 *entryt = sm + LZ_SM_ENTRY;
-	u32 *escan = (u32 *)(sm + LZ_SM_ESCAN);
 	u16 *gexit = (u16 *)(sm + LZ_SM_GEXIT);
 	u32 *freq = (u32 *)(sm + LZ_SM_FREQ);
 	u8 *lens = sm + LZ_SM_LENS;
-	u16 *codes = (u16 *)(sm + LZ_SM_CODES);
 	lz_vars *v = (lz_vars *)(sm + LZ_SM_VARS);
-	// block-flush scratch aliases the parse region R (never live at the same time)
-	u32 *stage = (u32 *)(sm + LZ_SM_R);				// 8 KiB
-	u16 *hsorted = (u16 *)(sm + LZ_SM_R);				// 288 * 2
-	u32 *hnodefreq = (u32 *)(sm + LZ_SM_R + 1024);			// 576 * 4
-	u16 *hparent = (u16 *)(sm + LZ_SM_R + 1024 + 2304);		// 576 * 2
-	u16 *osorted = (u16 *)(sm + LZ_SM_R + 4608);
-	u32 *onodefreq = (u32 *)(sm + LZ_SM_R + 4608 + 128);
-	u16 *oparent = (u16 *)(sm + LZ_SM_R + 4608 + 128 + 512);
-	u16 *items = (u16 *)(sm + LZ_SM_ITEMS);				// precode items (<= 320 + slack)
+	u32 *stage = (u32 *)(sm + LZ_SM_R);	// block emission staging (aliases the parse region R)
 	// per-position results of the current pass live in this CTA's global scratch
 	u8 *gs = a.scratch + 256 + (size_t)blockIdx.x * LZ_GS_BYTES;
 	u32 *res = (u32 *)(gs + LZ_GS_RES);	// per position: match length | (distance-1 | DP decision flag << 15) << 16
@@ -829,10 +744,8 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 	// barrier.
 	const bool pipe = !P.opt_iters;
 	u32 GW = LZ_WARPS, GT = LZ_THREADS;
-	auto gsync = [&]() {
-		if (GT < LZ_THREADS) LDB_BAR_SYNC(LZ_BAR_P, GT);
-		else __syncthreads();
-	};
+	auto grp = [&]() { return lz_group{tid, lane, warp, GW, GT}; };
+	auto gsync = [&]() { grp().sync(); };
 
 	if (tid == 0) {
 		v->tma_phase = 0;
@@ -865,37 +778,9 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		o.out = (u8 *)a.out_ptrs[c];
 		o.avail = a.out_avail[c];
 		o.obit = 0;
-		const u32 overhead = a.format == LDB_FMT_GZIP ? 18 : (a.format == LDB_FMT_ZLIB ? 6 : 0);
-		const u32 trailer = a.format == LDB_FMT_GZIP ? 8 : (a.format == LDB_FMT_ZLIB ? 4 : 0);
-		const u32 hdr_bytes = overhead - trailer;
-
-		// ---- tiny inputs and oversize chunks take the stored path (ref: deflate_compress.c:4041-4043)
-		const bool passthrough = n64 <= (size_t)(55 - 4 * a.level) || n64 > 0x7fff0000u;
-		bool fits = !(overhead && o.avail <= overhead);
-		if (passthrough || !fits) {
-			const size_t nblocks = n64 ? (n64 + 65534) / 65535 : 1;
-			fits = fits && (n64 + 5 * nblocks <= o.avail - overhead);
-			if (!fits) {
-				if (tid == 0) a.out_nbytes[c] = 0;
-				continue;
-			}
-			if (tid == 0) def_write_header(o.out, a.format, a.level);
-			u8 *dst = o.out + hdr_bytes;
-			for (size_t b = 0; b < nblocks; b++) {
-				size_t off = b * 65535;
-				u32 len = (u32)(n64 - off > 65535 ? 65535 : n64 - off);
-				if (tid == 0) {
-					dst[0] = (b + 1 == nblocks && final_piece) ? 1 : 0;
-					dst[1] = (u8)len; dst[2] = (u8)(len >> 8);
-					dst[3] = (u8)~len; dst[4] = (u8)(~len >> 8);
-				}
-				for (u32 i = tid; i < len; i += LZ_THREADS) dst[5 + i] = in[off + i];
-				dst += 5 + len;
-			}
-			if (tid == 0) {
-				u32 t = def_write_trailer(dst, a.format, a.checksums ? a.checksums[c] : 0, n64);
-				a.out_nbytes[c] = (size_t)(dst - o.out) + t;
-			}
+		const u32 hdr_bytes = ldb_hdr_bytes(a.format);
+		if (lz_stored_chunk(n64, o.avail, a.format, a.level)) {
+			def_write_stored_chunk(a, c, tid, LZ_THREADS);
 			continue;
 		}
 		const u32 n = (u32)n64 + dict;	// end of the frame
@@ -1103,13 +988,9 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			if (warp == 0) {
 				u32 run = 0;
 				for (u32 w0 = 0; w0 < nwin; w0 += 32) {
-					u32 w = w0 + lane;
-					u32 c = w < nwin ? (u32)__popc(vis[w]) : 0;
-					u32 incl = c;
-					for (int o2 = 1; o2 < 32; o2 <<= 1) {
-						u32 t = __shfl_up_sync(LDB_FULL_MASK, incl, o2);
-						if (lane >= (u32)o2) incl += t;
-					}
+					const u32 w = w0 + lane;
+					const u32 c = w < nwin ? (u32)__popc(vis[w]) : 0;
+					const u32 incl = lz_warp_incl_scan(c, lane);
 					if (w < nwin) tokoff[w] = run + incl - c;
 					run += __shfl_sync(LDB_FULL_MASK, incl, 31);
 				}
@@ -1149,122 +1030,6 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			}
 			gsync();
 			if (tid == 0) v->tok_count = tbase + tokoff[LZ_NWIN];
-			gsync();
-		};
-
-		// ---- Huffman codes from freq[] -> lens[], codes[] (all threads)
-		// CTA-wide exclusive scan (all threads must call it); escan[0..64] is the scratch
-		auto cta_excl_scan = [&](u32 x, u32 &total) -> u32 {
-			u32 incl = x;
-			for (int o2 = 1; o2 < 32; o2 <<= 1) {
-				u32 t = __shfl_up_sync(LDB_FULL_MASK, incl, o2);
-				if (lane >= (u32)o2) incl += t;
-			}
-			gsync();		// earlier readers of escan are done
-			if (lane == 31) escan[warp] = incl;
-			gsync();
-			if (warp == 0) {
-				u32 y = lane < GW ? escan[lane] : 0;
-				u32 yi = y;
-				for (int o2 = 1; o2 < 32; o2 <<= 1) {
-					u32 t = __shfl_up_sync(LDB_FULL_MASK, yi, o2);
-					if (lane >= (u32)o2) yi += t;
-				}
-				if (lane < GW) escan[32 + lane] = yi - y;
-				if (lane == GW - 1) escan[64] = yi;
-			}
-			gsync();
-			total = escan[64];
-			return escan[32 + warp] + (incl - x);
-		};
-		auto build_codes = [&]() {
-			// (f1) Huffman codes for both alphabets.  Parallel: rank sort by (freq, sym), leaf depths
-			// (every leaf walks to the root), length assignment, canonical codewords (rank among the
-			// symbols of equal length).  Serial: only the two-queue merges, on thread 0 (litlen)
-			// and thread 32 (offset), and the rare Kraft repair after the 15-bit cap.
-			u32 *hcount = (u32 *)(sm + LZ_SM_GEXIT + 256), *ocount = hcount + 17;	// codewords per length
-			const bool is_lit = tid < 288;
-			const u32 lo = is_lit ? 0 : 288, hi = is_lit ? 288 : 320;
-			if (tid == 0) { v->nused_lit = 0; v->nused_off = 0; v->huff_over = 0; }
-			if (tid < 34) hcount[tid] = 0;
-			gsync();
-			u32 myrank = 0xffffffffu;
-			if (tid < 320) {
-				const u32 f = freq[tid];
-				lens[tid] = 0;
-				if (f) {
-					u32 rank = 0;
-					for (u32 t = lo; t < hi; t++) {
-						u32 ft = freq[t];
-						rank += (ft != 0) && (ft < f || (ft == f && t < tid));
-					}
-					myrank = rank;
-					(is_lit ? hsorted : osorted)[rank] = (u16)(tid - lo);
-					(is_lit ? hnodefreq : onodefreq)[rank] = f;
-					atomicAdd(is_lit ? &v->nused_lit : &v->nused_off, 1u);
-				}
-			}
-			gsync();
-			const u32 nused = is_lit ? v->nused_lit : v->nused_off;
-			if (tid == 0 && nused >= 2) lz_huffman_merge(hnodefreq, hparent, nused);
-			if (tid == 32) { const u32 nu = v->nused_off; if (nu >= 2) lz_huffman_merge(onodefreq, oparent, nu); }
-			gsync();
-			if (tid < 320 && myrank != 0xffffffffu && nused >= 2) {
-				const u16 *par = is_lit ? hparent : oparent;
-				const u32 root = 2 * nused - 2;
-				u32 node = myrank, d = 0;
-				while (node != root && d <= 15) { node = par[node]; d++; }
-				if (d > 15) { d = 15; v->huff_over = 1; }
-				atomicAdd(&(is_lit ? hcount : ocount)[d], 1u);
-			}
-			gsync();
-			if ((tid == 0 || tid == 288) && nused < 2) {
-				// at least two codewords (ref: deflate_compress.c:1369-1378)
-				u8 *ln = lens + lo;
-				u32 *cn = is_lit ? hcount : ocount;
-				if (nused == 0) { ln[0] = 1; ln[1] = 1; }
-				else { const u32 sy = (is_lit ? hsorted : osorted)[0]; ln[sy] = 1; ln[sy ? 0 : 1] = 1; }
-				cn[1] = 2;
-			}
-			if ((tid == 0 || tid == 32) && v->huff_over) {
-				// restore the Kraft sum to exactly 1 by lengthening the cheapest leaves
-				u32 *cn = tid == 0 ? hcount : ocount;
-				u32 kraft = 0;
-				for (u32 l = 1; l <= 15; l++) kraft += cn[l] << (15 - l);
-				while (kraft > (1u << 15)) {
-					u32 l = 14;
-					while (cn[l] == 0) l--;
-					cn[l]--;
-					cn[l + 1] += 2;
-					cn[15]--;
-					kraft -= 1;
-				}
-			}
-			gsync();
-			if (tid < 320 && myrank != 0xffffffffu && nused >= 2) {
-				// rarest symbols get the longest codes
-				const u32 *cn = is_lit ? hcount : ocount;
-				u32 cum = 0, len = 1;
-				for (u32 l = 15; l >= 1; l--) {
-					cum += cn[l];
-					if (myrank < cum) { len = l; break; }
-				}
-				lens[tid] = (u8)len;
-			}
-			gsync();
-			if (tid < 320) {
-				const u32 l = lens[tid];
-				u32 code = 0;
-				if (l) {
-					const u32 *cn = is_lit ? hcount : ocount;
-					u32 first = 0;
-					for (u32 k = 1; k < l; k++) first = (first + cn[k]) << 1;
-					u32 same = 0;
-					for (u32 t = lo; t < tid; t++) same += lens[t] == l;
-					code = __brev(first + same) >> (32 - l);
-				}
-				codes[tid] = (u16)code;
-			}
 			gsync();
 		};
 
@@ -1386,9 +1151,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 			// previous parse; min-cost path by backward DP over independent 2048-position segments
 			// (one warp each); the resulting choices are re-parsed by the same parallel parser.
 			for (int it = 0; it < P.opt_iters; it++) {
-				if (tid == 0) freq[256] = 1;
-				gsync();
-				build_codes();
+				lz_build_codes(grp(), sm);
 				// bit costs: unused symbols get a pessimistic default (cf. deflate_compress.c:149-151)
 				for (u32 k = tid; k < 256 + 259 + 32; k += GT) {
 					u32 c;
@@ -1426,386 +1189,22 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					parse_pass(pb0, ppend, pp * LZ_PASS, true, nextt + ((block_begin + npass_block * LZ_PASS) & 0xffff));
 				}
 			}
-			const u32 ntok = v->tok_count;
-
-			// ======================= block flush =========================================
 			LZ_T(7);	// optimal-parse iterations
-			if (tid == 0) freq[256] = 1;
-			gsync();
-			build_codes();
+			const lz_group g = grp();
+			lz_build_codes(g, sm);
 			LZ_T(4);	// Huffman codes
-			// (f2) precode items + precode, ref: deflate_compress.c:1483-1631.  Run-length items in
-			// parallel: thread j looks at code length j of the hlit+hdist sequence, run starts are
-			// found with ballots, every start knows in closed form how many items its run becomes,
-			// a CTA scan places them.  Only the 19-symbol precode itself is built by one thread.
-			u32 *pfreq_sm = (u32 *)(sm + LZ_SM_GEXIT);		// u32[19] (region unused while flushing)
-			u8 *plens_sm = sm + LZ_SM_GEXIT + 128;			// u8[19]
-			u16 *pcodes_sm = (u16 *)(sm + LZ_SM_GEXIT + 160);	// u16[19]
-			if (tid == 0) {
-				u32 hlit = 288;
-				while (hlit > 257 && lens[hlit - 1] == 0) hlit--;
-				v->hlit = hlit;
-			}
-			if (tid == 32) {
-				u32 hdist = 32;
-				while (hdist > 1 && lens[288 + hdist - 1] == 0) hdist--;
-				v->hdist = hdist;
-			}
-			if (tid >= 64 && tid < 64 + 19) pfreq_sm[tid - 64] = 0;
-			gsync();
-			{
-				const u32 hlit = v->hlit, total = hlit + v->hdist;
-				const u32 j = tid;
-				const bool inb = j < total;
-				const u32 val = inb ? (j < hlit ? lens[j] : lens[288 + j - hlit]) : 0xff;
-				const u32 prv = (inb && j > 0) ? (j - 1 < hlit ? lens[j - 1] : lens[288 + j - 1 - hlit]) : 0xfe;
-				const bool isstart = inb && val != prv;
-				const u32 smask = __ballot_sync(LDB_FULL_MASK, isstart);
-				if (lane == 0 && warp < 10) escan[66 + warp] = smask;
-				gsync();
-				u32 run = 0, cnt = 0;
-				if (isstart) {
-					u32 nxt = total;
-					u32 m = lane == 31 ? 0 : (smask & ~((2u << lane) - 1));
-					if (m) nxt = warp * 32 + __ffs(m) - 1;
-					else {
-						for (u32 w = warp + 1; w < 10; w++) {
-							u32 mm = escan[66 + w];
-							if (mm) { nxt = w * 32 + __ffs(mm) - 1; break; }
-						}
-					}
-					run = nxt - j;
-					if (val == 0) {
-						u32 rem = run % 138;
-						cnt = run / 138 + (rem >= 3 ? 1 : rem);
-					} else if (run >= 4) {
-						u32 rem = (run - 1) % 6;
-						cnt = 1 + (run - 1) / 6 + (rem >= 3 ? 1 : rem);
-					} else cnt = run;
-				}
-				u32 ntot;
-				const u32 off = cta_excl_scan(cnt, ntot);
-				if (isstart) {
-					u32 ni = off;
-					if (val == 0) {
-						while (run >= 11) {
-							u32 r = run < 138 ? run : 138;
-							items[ni++] = (u16)(18 | ((r - 11) << 5));
-							atomicAdd(&pfreq_sm[18], 1u);
-							run -= r;
-						}
-						if (run >= 3) {
-							items[ni++] = (u16)(17 | ((run - 3) << 5));
-							atomicAdd(&pfreq_sm[17], 1u);
-							run = 0;
-						}
-					} else if (run >= 4) {
-						items[ni++] = (u16)val;
-						atomicAdd(&pfreq_sm[val], 1u);
-						run--;
-						while (run >= 3) {
-							u32 r = run < 6 ? run : 6;
-							items[ni++] = (u16)(16 | ((r - 3) << 5));
-							atomicAdd(&pfreq_sm[16], 1u);
-							run -= r;
-						}
-					}
-					if (run) atomicAdd(&pfreq_sm[val], run);
-					while (run) { items[ni++] = (u16)val; run--; }
-				}
-				if (tid == 0) v->n_items = ntot;
-			}
-			gsync();
-			if (warp == 0) {
-				// the 19-symbol precode, limited to 7 bits, by warp 0: lane = symbol.  Same construction
-				// as build_codes (rank sort, two-queue merge on lane 0, leaf depths, Kraft repair, lengths
-				// by rank, canonical codewords), with the counts per length packed into one u64.
-				u32 *pnodef = (u32 *)(sm + LZ_SM_GEXIT + 512);		// u32[38]
-				u16 *ppar = (u16 *)(sm + LZ_SM_GEXIT + 672);		// u16[38]
-				const u32 lt = (1u << lane) - 1;
-				const u32 f = lane < 19 ? pfreq_sm[lane] : 0;
-				const u32 usedm = __ballot_sync(LDB_FULL_MASK, f != 0);
-				const u32 nused = __popc(usedm);
-				u32 rank = 0;
-				for (u32 t = 0; t < 19; t++) {
-					const u32 ft = __shfl_sync(LDB_FULL_MASK, f, t);
-					rank += (ft != 0) && (ft < f || (ft == f && t < lane));
-				}
-				if (f) pnodef[rank] = f;
-				__syncwarp();
-				if (lane == 0 && nused >= 2) lz_huffman_merge(pnodef, ppar, nused);
-				__syncwarp();
-				u32 d = 0;
-				bool over = false;
-				if (f && nused >= 2) {
-					const u32 root = 2 * nused - 2;
-					u32 node = rank;
-					while (node != root && d <= 7) { node = ppar[node]; d++; }
-					if (d > 7) { d = 7; over = true; }
-				}
-				u64 cn = 0;		// codewords per length, 8 bits each
-				for (u32 l = 1; l <= 7; l++) cn |= (u64)__popc(__ballot_sync(LDB_FULL_MASK, d == l)) << (8 * l);
-				if (__any_sync(LDB_FULL_MASK, over)) {
-					u32 kraft = 0;
-					for (u32 l = 1; l <= 7; l++) kraft += (u32)((cn >> (8 * l)) & 0xff) << (7 - l);
-					while (kraft > (1u << 7)) {
-						u32 l = 6;
-						while (((cn >> (8 * l)) & 0xff) == 0) l--;
-						cn -= (u64)1 << (8 * l);
-						cn += (u64)2 << (8 * (l + 1));
-						cn -= (u64)1 << (8 * 7);
-						kraft -= 1;
-					}
-				}
-				u32 len = 0;
-				if (nused >= 2) {
-					if (f) {
-						u32 cum = 0;
-						len = 1;
-						for (u32 l = 7; l >= 1; l--) {
-							cum += (u32)((cn >> (8 * l)) & 0xff);
-							if (rank < cum) { len = l; break; }
-						}
-					}
-				} else {
-					// at least two codewords
-					const u32 sy = nused ? (u32)__ffs(usedm) - 1 : 0;
-					len = (lane == sy || lane == (sy ? 0u : 1u)) ? 1 : 0;
-					cn = (u64)2 << 8;
-				}
-				u32 first = 0;
-				for (u32 k = 1; k < len; k++) first = (first + (u32)((cn >> (8 * k)) & 0xff)) << 1;
-				const u32 samem = __match_any_sync(LDB_FULL_MASK, len);
-				const u32 code = len ? __brev(first + __popc(samem & lt)) >> (32 - len) : 0;
-				if (lane < 19) { plens_sm[lane] = (u8)len; pcodes_sm[lane] = (u16)code; }
-				__syncwarp();
-				const u8 perm[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-				const u32 nzm = __ballot_sync(LDB_FULL_MASK, lane < 19 && plens_sm[perm[lane < 19 ? lane : 0]] != 0);
-				u32 hclen = nzm ? 32 - __clz(nzm) : 0;
-				if (hclen < 4) hclen = 4;
-				u32 cost = f * len + (lane == 16 ? 2 * f : lane == 17 ? 3 * f : lane == 18 ? 7 * f : 0);
-				for (int o2 = 16; o2 > 0; o2 >>= 1) cost += __shfl_xor_sync(LDB_FULL_MASK, cost, o2);
-				if (lane == 0) {
-					v->cost_dyn = cost + 3 + 5 + 5 + 4 + 3 * hclen;
-					v->hclen = hclen;
-					v->cost_static = 3;
-					v->extra_bits = 0;
-				}
-			}
-			gsync();
+			lz_precode(g, sm);
 			LZ_T(5);	// precode
-			// (f3) symbol costs (ref: deflate_compress.c:1750-1808)
-			if (tid < 320) {
-				u32 f = freq[tid];
-				if (f) {
-					u32 dyn = f * lens[tid];
-					u32 extra = 0, st;
-					if (tid < 288) {
-						st = f * lz_static_litlen_len(tid);
-						if (tid >= 257) extra = f * lz_len_extra_bits(tid - 257);
-					} else {
-						st = f * 5;
-						extra = f * lz_off_extra_bits(tid - 288);
-					}
-					atomicAdd(&v->cost_dyn, dyn + extra);
-					atomicAdd(&v->cost_static, st + extra);
-				}
-			}
-			gsync();
-			const u32 cost_dyn = v->cost_dyn, cost_static = v->cost_static;
-			// The tokens of this block cover [block_entry, parse_entry): its first token starts where the
-			// previous block's last match ended and its own last match may run past block_end.  A
-			// stored block must cover exactly the same bytes.
+			// The tokens of this block cover [block_entry, parse_entry): its first token starts where the previous
+			// block's last match ended, its own last may run past block_end.  A stored block covers the same.
 			// (past the end of the input the parser's continuation point is only window-granular)
-			const u32 sbeg = block_entry, blen = (v->parse_entry < n ? v->parse_entry : n) - block_entry;
-			const u32 bitoff = (u32)(o.obit & 7);
-			const u32 stored_pieces = blen ? (blen + 65534) / 65535 : 1;
-			// first piece: 3 header bits + pad to a byte; later pieces start byte aligned
-			const u64 cost_stored = (u64)(((bitoff + 3 + 7) & ~7u) - bitoff) + 32 + (u64)8 * blen + (u64)(stored_pieces - 1) * 40;
-			u32 btype;	// ties: stored, then static, then dynamic (deflate_compress.c:1804-1808)
-			u64 best = cost_stored;
-			btype = DEFLATE_BLOCKTYPE_STORED;
-			if (cost_static < best) { best = cost_static; btype = DEFLATE_BLOCKTYPE_STATIC; }
-			if (cost_dyn < best) { best = cost_dyn; btype = DEFLATE_BLOCKTYPE_DYNAMIC; }
-			// single bounds check for the whole block (deflate_compress.c:1811-1814); a non-final piece
-			// ends with an empty stored block: 3 bits, the pad to a byte and 4 bytes, at most 5 bytes
-			const u64 need_bytes = (o.obit + best + 7) / 8 + (last ? (LZ_NONFINAL ? 5 : trailer) : 0);
-			if (need_bytes > o.avail) {
-				if (tid == 0) v->failed = 1;
-				gsync();
-				return;
-			}
-
-			// staging covers bits starting at word 'w0' of the output; word 0 is seeded with
-			// the partial word carried from the previous flush
-			u64 w0 = o.obit >> 5;
-			for (u32 k = tid; k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
-			gsync();
-			if (tid == 0) stage[0] = v->carry;
-			gsync();
-			if (btype == DEFLATE_BLOCKTYPE_STORED) {
-				// ---- stored: header bits via staging, raw bytes straight from the input
-				u32 src = sbeg;
-				for (u32 piece = 0; piece < stored_pieces; piece++) {
-					u32 len = blen - (src - sbeg) > 65535 ? 65535 : blen - (src - sbeg);
-					bool fin = last && !LZ_NONFINAL && piece + 1 == stored_pieces;
-					if (tid == 0) {
-						lz_stage_or(stage, (u32)(o.obit - (w0 << 5)), fin ? 1 : 0, 3);
-						u64 ob = (o.obit + 3 + 7) & ~(u64)7;
-						lz_stage_or(stage, (u32)(ob - (w0 << 5)), (u64)len | ((u64)(~len & 0xffff) << 16), 32);
-					}
-					o.obit = ((o.obit + 3 + 7) & ~(u64)7) + 32;
-					gsync();
-					// flush staging up to the (byte aligned) current position, byte granular
-					{
-						u64 bytes_end = o.obit >> 3, bytes_begin = w0 * 4;
-						for (u64 k = bytes_begin + tid; k < bytes_end; k += GT) {
-							u32 rel = (u32)(k - bytes_begin);
-							o.out[k] = (u8)(stage[rel >> 2] >> (8 * (rel & 3)));
-						}
-					}
-					gsync();
-					for (u32 k = tid; k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
-					u8 *dst = o.out + (o.obit >> 3);
-					for (u32 k = tid; k < len; k += GT) dst[k] = in[src + k];
-					src += len;
-					o.obit += (u64)len * 8;
-					gsync();
-					// re-seed staging word 0 with the bytes already written in the current word
-					w0 = o.obit >> 5;
-					if (tid == 0) {
-						u32 nb = (u32)((o.obit >> 3) & 3);
-						u32 wv = 0;
-						for (u32 k = 0; k < nb; k++) wv |= (u32)(*(volatile u8 *)(o.out + w0 * 4 + k)) << (8 * k);
-						stage[0] = wv;
-					}
-					gsync();
-				}
-			} else {
-				// ---- Huffman block --------------------------------------------------------
-				if (btype == DEFLATE_BLOCKTYPE_STATIC) {
-					for (u32 s = tid; s < 320; s += GT) lens[s] = s < 288 ? (u8)lz_static_litlen_len(s) : 5;
-					gsync();
-					if (tid == 0) lz_gen_codes_serial(lens, 288, codes);
-					if (tid == 32) lz_gen_codes_serial(lens + 288, 32, codes + 288);
-					gsync();
-				}
-				// header: fixed fields by thread 0, the precode items by one thread each (bit offsets
-				// from a CTA scan), directly into staging
-				u32 rel;
-				{
-					const u32 rb0 = (u32)(o.obit - (w0 << 5));
-					u32 rb = rb0 + 3;
-					if (tid == 0) lz_stage_or(stage, rb0, (last && !LZ_NONFINAL ? 1 : 0) | (btype << 1), 3);
-					if (btype == DEFLATE_BLOCKTYPE_DYNAMIC) {
-						const u32 hclen = v->hclen, nit = v->n_items;
-						if (tid == 0)
-							lz_stage_or(stage, rb, (v->hlit - 257) | ((v->hdist - 1) << 5) | ((hclen - 4) << 10), 14);
-						rb += 14;
-						if (tid < hclen) {
-							const u8 perm[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-							lz_stage_or(stage, rb + 3 * tid, plens_sm[perm[tid]], 3);
-						}
-						rb += 3 * hclen;
-						u32 nb = 0, bits = 0;
-						if (tid < nit) {
-							const u32 it = items[tid], sym = it & 31, ex = it >> 5;
-							const u32 pl = plens_sm[sym];
-							const u32 eb = sym == 16 ? 2 : (sym == 17 ? 3 : (sym == 18 ? 7 : 0));
-							bits = pcodes_sm[sym] | (ex << pl);
-							nb = pl + eb;
-						}
-						u32 hbits;
-						const u32 hoff = cta_excl_scan(nb, hbits);
-						lz_stage_or(stage, rb + hoff, bits, nb);
-						rb += hbits;
-					}
-					rel = rb;	// bits used in staging so far (relative to word w0)
-				}
-				gsync();
-				// token rounds: bit lengths -> exclusive scan -> OR into staging -> flush whole words
-				const u32 tpt = LZ_TPT(GT);
-				for (u32 t0 = 0; t0 <= ntok; t0 += GT * tpt) {
-					// (the EOB symbol is token index ntok)
-					u32 mybits[2] = {};
-					u64 myval[2] = {};
-#pragma unroll
-					for (u32 r = 0; r < 2; r++) {
-						u32 ti = r < tpt ? t0 + tid * tpt + r : 0xffffffffu;
-						if (ti < ntok) {
-							u32 tk = tokbuf[ti];
-							if (tk & 0x80000000u) {
-								u32 len = ((tk >> 15) & 0x1ff) + 3, off = (tk & 0x7fff) + 1;
-								u32 ls = lz_len_slot(len), os = lz_off_slot(off);
-								u32 nb = lens[257 + ls];
-								u64 val = codes[257 + ls];
-								u32 leb = lz_len_extra_bits(ls);
-								val |= (u64)(len - lz_len_base(ls)) << nb;
-								nb += leb;
-								val |= (u64)codes[288 + os] << nb;
-								nb += lens[288 + os];
-								u32 oeb = lz_off_extra_bits(os);
-								val |= (u64)(off - lz_off_base(os)) << nb;
-								nb += oeb;
-								mybits[r] = nb;
-								myval[r] = val;
-							} else {
-								mybits[r] = lens[tk];
-								myval[r] = codes[tk];
-							}
-						} else if (ti == ntok) {
-							mybits[r] = lens[256];
-							myval[r] = codes[256];
-						}
-					}
-					// CTA-wide exclusive scan of the threads' bit counts
-					u32 mine = 0;
-#pragma unroll
-					for (u32 r = 0; r < 2; r++) mine += mybits[r];
-					u32 incl = mine;
-					for (int o2 = 1; o2 < 32; o2 <<= 1) {
-						u32 t = __shfl_up_sync(LDB_FULL_MASK, incl, o2);
-						if (lane >= (u32)o2) incl += t;
-					}
-					if (lane == 31) escan[warp] = incl;
-					gsync();
-					if (warp == 0) {
-						u32 x = lane < GW ? escan[lane] : 0;
-						u32 xi = x;
-						for (int o2 = 1; o2 < 32; o2 <<= 1) {
-							u32 t = __shfl_up_sync(LDB_FULL_MASK, xi, o2);
-							if (lane >= (u32)o2) xi += t;
-						}
-						if (lane < GW) escan[32 + lane] = xi - x;
-						if (lane == GW - 1) escan[64] = xi;
-					}
-					gsync();
-					u32 bitpos = rel + escan[32 + warp] + (incl - mine);
-#pragma unroll
-					for (u32 r = 0; r < 2; r++) {
-						lz_stage_or(stage, bitpos, myval[r], mybits[r]);
-						bitpos += mybits[r];
-					}
-					const u32 round_bits = escan[64];
-					gsync();
-					rel += round_bits;
-					// flush complete words, keep the partial one as the new stage[0]
-					u32 full = rel >> 5;
-					if (full) {
-						lz_flush_words(o, stage, w0, full, GT);
-						gsync();
-						u32 carry = stage[full];
-						gsync();
-						for (u32 k = tid; k <= full && k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
-						gsync();
-						if (tid == 0) stage[0] = carry;
-						w0 += full;
-						rel &= 31;
-						gsync();
-					}
-				}
-				o.obit = (w0 << 5) + rel;
-			}
+			const u32 blen = (v->parse_entry < n ? v->parse_entry : n) - block_entry;
+			// (a non-final piece ends with an empty stored block: at most 5 bytes)
+			const u32 btype = lz_block_choose(g, sm, o, blen, last ? (LZ_NONFINAL ? 5 : ldb_trl_bytes(a.format)) : 0);
+			if (btype == LZ_NOFIT) return;
+			lz_stage_reset(g, stage, o, &v->carry);
+			if (btype == DEFLATE_BLOCKTYPE_STORED) lz_emit_stored(g, sm, o, in + block_entry, blen, last && !LZ_NONFINAL);
+			else lz_emit_huffman(g, sm, o, tokbuf, v->tok_count, btype, last && !LZ_NONFINAL);
 			gsync();
 			if (tid == 0) v->carry = stage[0];
 			LZ_T(6);	// costs + emission
@@ -1823,41 +1222,6 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		// link slots of pass k + 2: insert(k + 1) used them as list scratch and is done with them, and no
 		// chain of pass k + 1 reaches that far back (they belong to positions >= 48 Ki back).
 		// (the passes of the dictionary, step < LZ_DICT / LZ_PASS, are only loaded and inserted)
-		// ---- final partial byte + trailer, by the group [0, GT); a chunk that did not fit gets size 0
-		auto finish = [&]() {
-			if (v->failed) {
-				if (tid == 0) a.out_nbytes[c] = 0;
-				return;
-			}
-			u64 w0 = o.obit >> 5;
-			for (u32 k = tid; k < LZ_STAGE_WORDS; k += GT) stage[k] = 0;
-			gsync();
-			if (tid == 0) stage[0] = v->carry;
-			gsync();
-			u64 ob;
-			if (!LZ_NONFINAL) {
-				ob = (o.obit + 7) & ~(u64)7;	// pad the last byte with zero bits
-				if (tid == 0 && trailer) {
-					u8 t[8];
-					def_write_trailer(t, a.format, a.checksums ? a.checksums[c] : 0, n64);
-					for (u32 k = 0; k < trailer; k++) lz_stage_or(stage, (u32)(ob - (w0 << 5)) + 8 * k, t[k], 8);
-				}
-				ob += (u64)trailer * 8;
-			} else {
-				// empty stored block (BFINAL 0, BTYPE 00, zero pad, LEN 0000, NLEN FFFF): the piece ends on a byte
-				ob = (o.obit + 3 + 7) & ~(u64)7;
-				if (tid == 0) lz_stage_or(stage, (u32)(ob - (w0 << 5)), 0xffff0000u, 32);
-				ob += 32;
-			}
-			gsync();
-			u64 bytes_begin = w0 * 4, bytes_end = ob >> 3;
-			for (u64 k = bytes_begin + tid; k < bytes_end; k += GT) {
-				u32 rel = (u32)(k - bytes_begin);
-				o.out[k] = (u8)(stage[rel >> 2] >> (8 * (rel & 3)));
-			}
-			if (tid == 0) a.out_nbytes[c] = (size_t)(ob >> 3);
-		};
-
 		// Hand-over (levels 1-9, batch instance): a chunk of 4k passes (64 KiB, 128 KiB, ...) parses its last
 		// pass in ring slots [48 Ki, 64 Ki), clear of the [0, 32 Ki + 16) that a chunk's step 0 loads.  Its
 		// step npass - 1 fetches the next chunk's index; if that chunk takes the LZ path, the last step runs
@@ -1885,7 +1249,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 				if (c1 < a.n) {
 					const size_t m64 = a.in_nbytes[c1];
 					n1 = (u32)m64;
-					beside = !(m64 <= (size_t)(55 - 4 * a.level) || m64 > 0x7fff0000u) && !(overhead && a.out_avail[c1] <= overhead);
+					beside = !lz_stored_chunk(m64, a.out_avail[c1], a.format, a.level);
 				}
 			}
 			const u32 hw = a.pwarps[2];			// hand-over: warps of the parse/flush group
@@ -1987,7 +1351,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 					const u32 kb0 = b0 - LZ_PASS;
 					parse_and_flush(kb0, kb0 + LZ_PASS < n ? kb0 + LZ_PASS : n, ((step - 1) & 1) * LZ_PASS,
 							nextt + ((kb0 + (beside ? 0 : 2 * LZ_PASS)) & 0xffff));
-					if (beside) finish();
+					if (beside) lz_finish(grp(), sm, a, c, o, LZ_NONFINAL);
 					LZ_TSPLIT_BUSY();
 					if (beside) LDB_BAR_SYNC(LZ_BAR_H, LZ_THREADS);	// the next chunk's insert(0) is done
 				}
@@ -2025,7 +1389,7 @@ ldb_deflate_lz_kernel(ldb_deflate_args a)
 		__syncthreads();
 		GW = LZ_WARPS;
 		GT = LZ_THREADS;
-		finish();
+		lz_finish(grp(), sm, a, c, o, LZ_NONFINAL);
 		__syncthreads();
 		LZ_T(7);	// chunk prologue/epilogue
 	}

@@ -934,7 +934,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 		}
 		int verdict = (int)s.verdict;
 		const u32 out_pos = inf_out_pos(s);
-		u32 footer = a.format == LDB_FMT_GZIP ? 8 : (a.format == LDB_FMT_ZLIB ? 4 : 0);
+		u32 footer = ldb_trl_bytes(a.format);
 		if (verdict == LDB_SUCCESS) {
 			u64 P = inf_bits_consumed(s);
 			if (P > (u64)s.in_n * 8) verdict = LDB_BAD_DATA;	// decompress_template.h:754
@@ -1019,7 +1019,7 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 							s.pfx = pfx;
 							s.reach = 0;
 							s.split_i = g.split_i[c];
-							u32 footer = a.format == LDB_FMT_GZIP ? 8 : (a.format == LDB_FMT_ZLIB ? 4 : 0);
+							u32 footer = ldb_trl_bytes(a.format);
 							u64 skip = st >> 3;
 							if (st == 0) {	// the stream start: the wrapper header is parsed here only
 								const u32 hdr = inf_parse_wrapper(g.base, g.in_nbytes, a.format, &footer);

@@ -17,8 +17,6 @@
 // written once.
 #include "ldb_common.cuh"
 
-__device__ __forceinline__ u32 lg_trl_bytes(int format) { return format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0); }
-
 __global__ void __launch_bounds__(256)
 ldb_large_setup_kernel(ldb_large_args a)
 {
@@ -113,7 +111,7 @@ ldb_large_plan_kernel(ldb_large_args a)
 		__syncthreads();
 	}
 	if (tid == LG_PLAN_THREADS - 1) {	// (its pos is the end of the wave)
-		const u32 hdr = a.hdr, trl = a.final_piece ? lg_trl_bytes(a.format) : 0;
+		const u32 hdr = a.hdr, trl = a.final_piece ? ldb_trl_bytes(a.format) : 0;
 		const u64 total = pos;
 		const u32 failed = st.failed || any_empty || (u64)hdr + total + trl > a.out_avail;
 		const u32 run = ck ? ldb_sum_combine(a.format, xp, st.sum, tv[0], tl[0]) : 0;

@@ -76,6 +76,11 @@ typedef int32_t s32;
 #define DEFLATE_MAX_CODEWORD_LEN   15
 #define DEFLATE_MAX_PRE_CODEWORD_LEN 7
 
+// Wrapper header and trailer bytes per format (ref: gzip_compress.c:32-80, zlib_compress.c:32-72).
+__host__ __device__ __forceinline__ u32 ldb_hdr_bytes(int format) { return format == LDB_FMT_GZIP ? 10 : (format == LDB_FMT_ZLIB ? 2 : 0); }
+__host__ __device__ __forceinline__ u32 ldb_trl_bytes(int format) { return format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0); }
+__host__ __device__ __forceinline__ u32 ldb_wrap_bytes(int format) { return ldb_hdr_bytes(format) + ldb_trl_bytes(format); }
+
 // Writes the wrapper header at out, returns its size (ref: gzip_compress.c:43-62,
 // zlib_compress.c:45-63).  Used by the deflate kernels and by the stream stitch (large_kernels.cu).
 __device__ __forceinline__ u32 def_write_header(u8 *out, int format, int level)
@@ -312,6 +317,40 @@ struct ldb_deflate_args {
 };
 #define LDB_PIECE_NONFINAL 0x80000000u
 #define LDB_PIECE_DICT_MASK 0x7fffffffu
+// Chunk c of a as stored blocks of <= 65,535 bytes in its wrapper (ref: deflate_compress_none, deflate_compress.c:
+// 2393-2443), by threads [0, nthreads); out_nbytes[c] = 0 if they do not fit.  A non-final piece of a larger
+// stream only lacks BFINAL: stored blocks end byte-aligned.
+__device__ __forceinline__ void def_write_stored_chunk(const ldb_deflate_args &a, size_t c, u32 tid, u32 nthreads)
+{
+	const u8 *in = (const u8 *)a.in_ptrs[c];
+	const size_t n = a.in_nbytes[c], avail = a.out_avail[c];
+	u8 *out = (u8 *)a.out_ptrs[c];
+	const u32 overhead = ldb_wrap_bytes(a.format);
+	const size_t nblocks = n ? (n + 65534) / 65535 : 1;
+	// the wrappers refuse avail <= overhead outright (gzip_compress.c:40, zlib_compress.c:42)
+	if ((overhead && avail <= overhead) || n + 5 * nblocks > avail - overhead) {
+		if (tid == 0) a.out_nbytes[c] = 0;
+		return;
+	}
+	if (tid == 0) def_write_header(out, a.format, a.level);
+	const bool final_piece = !(a.piece && (a.piece[c] & LDB_PIECE_NONFINAL));
+	u8 *dst = out + ldb_hdr_bytes(a.format);
+	for (size_t b = 0; b < nblocks; b++) {
+		const size_t off = b * 65535;
+		const u32 len = (u32)(n - off > 65535 ? 65535 : n - off);
+		if (tid == 0) {
+			dst[0] = (b + 1 == nblocks && final_piece) ? 1 : 0;	// BFINAL, BTYPE = 00
+			dst[1] = (u8)len; dst[2] = (u8)(len >> 8);
+			dst[3] = (u8)~len; dst[4] = (u8)(~len >> 8);
+		}
+		for (u32 i = tid; i < len; i += nthreads) dst[5 + i] = in[off + i];
+		dst += 5 + len;
+	}
+	if (tid == 0) {
+		const u32 t = def_write_trailer(dst, a.format, a.checksums ? a.checksums[c] : 0, n);
+		a.out_nbytes[c] = (size_t)(dst - out) + t;
+	}
+}
 int ldb_launch_deflate(const ldb_deflate_args &a, const ldb_launch_cfg &cfg, void *stream);
 size_t ldb_deflate_scratch_bytes(const ldb_launch_cfg &cfg, size_t n);
 int ldb_deflate_grid(const ldb_launch_cfg &cfg);

@@ -379,7 +379,6 @@ static int check_level(int *level)
 }
 
 // bytes the zlib / gzip wrapper adds to a raw DEFLATE stream
-static size_t wrap_bytes(int format) { return format == LDB_FMT_GZIP ? 18 : (format == LDB_FMT_ZLIB ? 6 : 0); }
 
 // a positive integer from the environment; dflt when the variable is unset or not positive
 static size_t ldb_env_size(const char *name, size_t dflt)
@@ -934,7 +933,7 @@ extern "C" int libdeflate_b200_compress_batch_host_packed(struct libdeflate_b200
 	size_t slots = 0;
 	for (size_t i = 0; i < n; i++) {
 		slot_off[i] = slots;
-		slots += align_up(wrap_bytes(format) + ldb_raw_bound(h_in_nbytes[i]), 16);
+		slots += align_up(ldb_wrap_bytes(format) + ldb_raw_bound(h_in_nbytes[i]), 16);
 	}
 	slot_off[n] = slots;
 	// parameter block: in ptrs/sizes | out ptrs/avail | out sizes | offsets (n + 1 u64, per sub-batch)
@@ -1071,10 +1070,10 @@ static int read_back(libdeflate_b200_ctx *ctx, void *h, const void *d, size_t nb
 // ---------------------------------------------------------------------------------
 extern "C" size_t libdeflate_b200_compress_large_bound(int format, size_t in_nbytes)
 {
-	if (in_nbytes <= LDB_LARGE_PIECE) return wrap_bytes(format) + ldb_raw_bound(in_nbytes);
+	if (in_nbytes <= LDB_LARGE_PIECE) return ldb_wrap_bytes(format) + ldb_raw_bound(in_nbytes);
 	// every piece fits its raw bound; all but the last add their closing empty stored block
 	const size_t full = (in_nbytes - 1) / LDB_LARGE_PIECE;
-	return wrap_bytes(format) + full * (ldb_raw_bound(LDB_LARGE_PIECE) + 5) + ldb_raw_bound(in_nbytes - full * LDB_LARGE_PIECE);
+	return ldb_wrap_bytes(format) + full * (ldb_raw_bound(LDB_LARGE_PIECE) + 5) + ldb_raw_bound(in_nbytes - full * LDB_LARGE_PIECE);
 }
 
 // Pieces per wave (default 1 GiB of input; LIBDEFLATE_B200_LARGE_WAVE_KB overrides): the context keeps the
@@ -1084,7 +1083,6 @@ static size_t large_wave_pieces(void)
 	return std::max((ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_KB", (size_t)1 << 20) << 10) / LDB_LARGE_PIECE, (size_t)1);
 }
 
-static u32 hdr_bytes(int format) { return format == LDB_FMT_GZIP ? 10 : (format == LDB_FMT_ZLIB ? 2 : 0); }
 
 // The context's per-wave room for waves of up to 'wave' pieces -- ctx->large: in_ptrs | in_nbytes | out_ptrs |
 // out_avail | out_nbytes | offsets | piece | sums | state | slots, and the deflate scratch (slots = false: one
@@ -1158,7 +1156,7 @@ extern "C" int libdeflate_b200_compress_large(struct libdeflate_b200_ctx *ctx, i
 	g.out_nbytes = d_out_nbytes;
 	g.format = format;
 	g.level = level;
-	g.hdr = hdr_bytes(format);
+	g.hdr = ldb_hdr_bytes(format);
 	g.direct = npieces == 1;	// the whole input is one chunk
 	for (size_t first = 0; first < npieces; first += wave) {
 		const size_t off = first * LDB_LARGE_PIECE;
@@ -1236,7 +1234,7 @@ static cs_plan cs_plan_of(const libdeflate_b200_compress_stream *s, size_t n, in
 		p.emit = t;
 		p.pieces = 1;
 		p.direct = true;
-		p.bound = wrap_bytes(s->format) + ldb_raw_bound(t);
+		p.bound = ldb_wrap_bytes(s->format) + ldb_raw_bound(t);
 		return p;
 	}
 	// without a flush a complete piece waits for one more byte: only then is it known not to be final
@@ -1247,8 +1245,8 @@ static cs_plan cs_plan_of(const libdeflate_b200_compress_stream *s, size_t n, in
 	// every piece fits its raw bound; the non-final ones add their closing empty stored block
 	const size_t last = p.emit - (p.pieces - 1) * P;
 	p.bound = (p.pieces - 1) * (ldb_raw_bound(P) + 5) + ldb_raw_bound(last) + (p.fin ? 0 : 5);
-	if (!s->started) p.bound += hdr_bytes(s->format);
-	if (p.fin) p.bound += wrap_bytes(s->format) - hdr_bytes(s->format);
+	if (!s->started) p.bound += ldb_hdr_bytes(s->format);
+	if (p.fin) p.bound += ldb_trl_bytes(s->format);
 	return p;
 }
 
@@ -1329,7 +1327,7 @@ static int cs_write(libdeflate_b200_compress_stream *s, const void *in, size_t n
 	g.out_nbytes = d_out_nbytes;
 	g.format = s->format;
 	g.level = s->level;
-	g.hdr = s->started ? 0 : hdr_bytes(s->format);
+	g.hdr = s->started ? 0 : ldb_hdr_bytes(s->format);
 	g.direct = p.direct;
 	const u64 before = s->total - s->pending;	// stream bytes before the call's first piece
 	size_t used = 0, hist = s->hist, bytes = 0;	// input bytes staged; history and piece bytes of the wave
@@ -1596,7 +1594,7 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	const u8 *in = (const u8 *)d_in;
 	u8 *out = (u8 *)d_out;
 	const size_t n = in_nbytes;
-	const u32 footer = format == LDB_FMT_GZIP ? 8 : (format == LDB_FMT_ZLIB ? 4 : 0);
+	const u32 footer = ldb_trl_bytes(format);
 	const u64 data_end = n >= footer ? n - footer : 0;	// the DEFLATE data ends before the trailer
 
 	// ---- 1. split points: sync points, else found block starts -----------------------------------------
@@ -1904,8 +1902,8 @@ extern "C" size_t libdeflate_b200_bgzf_compress_bound(size_t in_nbytes)
 {
 	const size_t B = LIBDEFLATE_B200_BGZF_BLOCK;
 	const size_t full = in_nbytes / B, tail = in_nbytes % B;
-	size_t total = full * (wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(B) + 8) + sizeof(LDB_BGZF_EOF);
-	if (tail) total += wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(tail) + 8;
+	size_t total = full * (ldb_wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(B) + 8) + sizeof(LDB_BGZF_EOF);
+	if (tail) total += ldb_wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(tail) + 8;
 	return total;
 }
 
@@ -1914,7 +1912,7 @@ extern "C" int libdeflate_b200_bgzf_compress(struct libdeflate_b200_ctx *ctx, in
 {
 	const size_t B = LIBDEFLATE_B200_BGZF_BLOCK;
 	const size_t nblk = (in_nbytes + B - 1) / B;
-	const size_t slot = (wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(B) + 15) & ~(size_t)15;
+	const size_t slot = (ldb_wrap_bytes(LDB_FMT_GZIP) + ldb_raw_bound(B) + 15) & ~(size_t)15;
 	*out_nbytes = 0;
 	size_t pos = 0;
 	u8 *o = (u8 *)out;
@@ -2106,11 +2104,11 @@ extern "C" size_t libdeflate_deflate_compress_bound(struct libdeflate_compressor
 }
 extern "C" size_t libdeflate_zlib_compress_bound(struct libdeflate_compressor *c, size_t in_nbytes)
 {
-	return wrap_bytes(LDB_FMT_ZLIB) + libdeflate_deflate_compress_bound(c, in_nbytes);
+	return ldb_wrap_bytes(LDB_FMT_ZLIB) + libdeflate_deflate_compress_bound(c, in_nbytes);
 }
 extern "C" size_t libdeflate_gzip_compress_bound(struct libdeflate_compressor *c, size_t in_nbytes)
 {
-	return wrap_bytes(LDB_FMT_GZIP) + libdeflate_deflate_compress_bound(c, in_nbytes);
+	return ldb_wrap_bytes(LDB_FMT_GZIP) + libdeflate_deflate_compress_bound(c, in_nbytes);
 }
 
 static bool is_device_pointer(const void *p)

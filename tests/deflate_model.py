@@ -1,5 +1,5 @@
 """A plain model of the deflate kernel's block encoder, and a table-driven disassembler to hold its
-streams against it (deflate_lz_kernel.cuh: build_codes, the precode step (f2), the block costs (f3)).
+streams against it (deflate_block.cuh: lz_build_codes, lz_precode (f2), lz_block_choose (f3)).
 
 The model restates the kernel's documented rules, not any other encoder's:
   * Huffman code: leaves sorted by (freq, symbol), two-queue merge (a leaf wins a tie with an internal
