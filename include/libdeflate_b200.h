@@ -343,6 +343,66 @@ libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx *ctx, int forma
 LIBDEFLATEAPI size_t
 libdeflate_b200_decompress_large_segments(struct libdeflate_b200_ctx *ctx);
 
+/*
+ * ONE DEFLATE / zlib / gzip stream read call by call, zlib's inflate() loop: input that arrives over time or
+ * does not fit in device memory.  Each call decodes what it can with decompress_large's chain of segments,
+ * started from the stream's carried 32 KiB window instead of the stream start.
+ *
+ * Input: a call takes all of its input and appends it to the input the stream holds (unless it returns an
+ *   error code: then the stream is unchanged).
+ * Output: a call writes to out the output of the stream's COMPLETE blocks that it has not delivered yet, in
+ *   order, as many whole blocks as fit in out_avail.  A block is complete when its last bit (the end of its
+ *   end-of-block code, or of its stored data) lies within the input written so far.  Output is never
+ *   delivered from inside a block; the final block's output is delivered once it is complete, even before its
+ *   trailer arrives.  *out_nbytes is what this call wrote.
+ * *result (host):
+ *   LIBDEFLATE_SUCCESS: the stream ended, its trailer checked (CRC-32 and ISIZE mod 2^32, or Adler-32), and
+ *     all of its output is delivered.  *in_unused is the number of input bytes written that lie after the
+ *     stream's end (a next gzip member starts there).
+ *   LIBDEFLATE_BAD_DATA: the stream is malformed, its trailer does not match, or 'last' was set and the
+ *     stream had not ended once every complete block was delivered.
+ *   LIBDEFLATE_B200_MORE_INPUT: every complete block is delivered; the stream needs more input.
+ *   LIBDEFLATE_B200_MORE_OUTPUT: complete blocks remain undelivered; call again.  *out_needed is the room the
+ *     next undelivered block needs (out_avail = 0 is legal).
+ *   After SUCCESS or BAD_DATA every later write returns an error code (last_error() says "finished").
+ *   out_needed and in_unused may be NULL.
+ * Equivalence: cut any stream into writes, set 'last' on the final one and call until MORE_OUTPUT stops:
+ *   the final result is decompress_large's on the whole buffer with ample out_avail, and on SUCCESS so are
+ *   the concatenated output, actual_out and actual_in (= input written - *in_unused).  A valid stream cut
+ *   short, with 'last' never set, never gives BAD_DATA: a decode that needs bits past the input means
+ *   "not complete yet".
+ *
+ * decompress_stream_create: NULL (last_error() says why) on a bad format.  No preset dictionaries (zlib
+ *   FDICT is BAD_DATA).
+ * decompress_stream_pending: the input bytes the stream holds, from the byte that contains the first
+ *   undelivered block's first bit: its memory bound.  Besides them it keeps only its last <= 32 KiB of output,
+ *   the running checksum and length, and whether the wrapper header is parsed; all per-call scratch belongs
+ *   to the context, so many streams can share one.
+ * decompress_stream_write: device pointers.  It WAITS on the context's stream, as decompress_large does, and
+ *   its results are host values.  Nothing is written outside [out, out + out_avail), and the input is never
+ *   written.
+ * decompress_stream_write_host: host buffers, staging included.
+ * Limits as for decompress_large: a segment has less than 4 GiB - 16 bytes of input and 4 GiB - 32 KiB of
+ * output.  Kernel time as for decompress_large.
+ */
+#define LIBDEFLATE_B200_MORE_INPUT   0x100
+#define LIBDEFLATE_B200_MORE_OUTPUT  0x101
+struct libdeflate_b200_decompress_stream;
+LIBDEFLATEAPI struct libdeflate_b200_decompress_stream *
+libdeflate_b200_decompress_stream_create(struct libdeflate_b200_ctx *ctx, int format);
+LIBDEFLATEAPI void
+libdeflate_b200_decompress_stream_destroy(struct libdeflate_b200_decompress_stream *s);
+LIBDEFLATEAPI size_t
+libdeflate_b200_decompress_stream_pending(const struct libdeflate_b200_decompress_stream *s);
+LIBDEFLATEAPI int
+libdeflate_b200_decompress_stream_write(struct libdeflate_b200_decompress_stream *s,
+					const void *d_in, size_t in_nbytes, int last, void *d_out, size_t out_avail,
+					size_t *out_nbytes, size_t *out_needed, size_t *in_unused, int32_t *result);
+LIBDEFLATEAPI int
+libdeflate_b200_decompress_stream_write_host(struct libdeflate_b200_decompress_stream *s,
+					     const void *in, size_t in_nbytes, int last, void *out, size_t out_avail,
+					     size_t *out_nbytes, size_t *out_needed, size_t *in_unused, int32_t *result);
+
 #ifdef __cplusplus
 }
 #endif

@@ -53,9 +53,14 @@ BATCH_SYMBOLS = [
     "libdeflate_b200_decompress_large", "libdeflate_b200_decompress_large_host", "libdeflate_b200_decompress_large_segments",
     "libdeflate_b200_compress_stream_create", "libdeflate_b200_compress_stream_destroy", "libdeflate_b200_compress_stream_bound",
     "libdeflate_b200_compress_stream_write", "libdeflate_b200_compress_stream_write_host",
+    "libdeflate_b200_decompress_stream_create", "libdeflate_b200_decompress_stream_destroy",
+    "libdeflate_b200_decompress_stream_pending", "libdeflate_b200_decompress_stream_write",
+    "libdeflate_b200_decompress_stream_write_host",
 ]
 LARGE_PIECE = 131072    # LIBDEFLATE_B200_LARGE_PIECE: input bytes per piece of compress_large
 NO_FLUSH, SYNC_FLUSH, FINISH = 0, 1, 2     # flush modes of a compress stream's write
+SUCCESS, BAD_DATA = 0, 1                   # libdeflate results
+MORE_INPUT, MORE_OUTPUT = 0x100, 0x101     # the other results of a decompress stream's write
 
 
 class Options(ctypes.Structure):
@@ -186,6 +191,16 @@ def load_library(path=None):
     lib.libdeflate_b200_compress_stream_write.argtypes = [P, P, S, c_int, P, S, P]
     lib.libdeflate_b200_compress_stream_write_host.restype = c_int
     lib.libdeflate_b200_compress_stream_write_host.argtypes = [P, P, S, c_int, P, S, PS]
+    lib.libdeflate_b200_decompress_stream_create.restype = P
+    lib.libdeflate_b200_decompress_stream_create.argtypes = [P, c_int]
+    lib.libdeflate_b200_decompress_stream_destroy.restype = None
+    lib.libdeflate_b200_decompress_stream_destroy.argtypes = [P]
+    lib.libdeflate_b200_decompress_stream_pending.restype = S
+    lib.libdeflate_b200_decompress_stream_pending.argtypes = [P]
+    for f in ("write", "write_host"):
+        fn = getattr(lib, "libdeflate_b200_decompress_stream_" + f)
+        fn.restype = c_int
+        fn.argtypes = [P, P, S, c_int, P, S, PS, PS, PS, POINTER(c_int32)]
     return lib
 
 
@@ -438,6 +453,10 @@ class Context:
         """A CompressStream on this context: ONE stream written call by call, like zlib.compressobj."""
         return CompressStream(self, level, fmt)
 
+    def decompressobj(self, fmt=RAW):
+        """A DecompressStream on this context: ONE stream read call by call, like zlib.decompressobj."""
+        return DecompressStream(self, fmt)
+
     def large_segments(self):
         """Segments the last decompress_large decoded in parallel (1: one lane)."""
         return self.l.libdeflate_b200_decompress_large_segments(self.h)
@@ -560,6 +579,116 @@ class CompressStream:
     def close(self):
         if self.h:
             self.l.libdeflate_b200_compress_stream_destroy(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class DecompressStream:
+    """libdeflate_b200_decompress_stream, shaped like zlib.decompressobj: decompress(data, max_length=0) ->
+    bytes, flush() -> bytes (a write of nothing with 'last' set), eof, unused_data, pending.  Every call decodes
+    the complete blocks it can with the whole GPU.  Host buffers."""
+
+    def __init__(self, ctx, fmt=RAW):
+        self.ctx = ctx
+        self.l = ctx.l
+        self.h = self.l.libdeflate_b200_decompress_stream_create(ctx.h, fmt)
+        if not self.h:
+            raise Error("decompress_stream_create(fmt=%d) failed: %s" % (fmt, self.l.libdeflate_b200_last_error().decode()))
+        ctx._streams.add(self)
+        self.eof = False
+        self.unused_data = b""
+        self.result = None      # the last write's result
+        self.needed = 0         # after MORE_OUTPUT: the room the next block needs
+        self._room = 1 << 16
+        self._buf = b""
+        self._recent = b""
+
+    @property
+    def pending(self):
+        return self.l.libdeflate_b200_decompress_stream_pending(self.h) if self.h else 0
+
+    def write(self, data, last=False, out_avail=None):
+        """One write_host call: (result, output bytes, out_needed, in_unused)."""
+        if not self.h:
+            raise Error("decompress stream is closed")
+        addr, n, keep = _buf_ptr(data)
+        avail = self._room if out_avail is None else out_avail
+        out = ctypes.create_string_buffer(max(avail, 1))
+        w, need, unused, res = c_size_t(0), c_size_t(0), c_size_t(0), c_int32(0)
+        rc = self.l.libdeflate_b200_decompress_stream_write_host(self.h, addr, n, 1 if last else 0, out, avail, ctypes.byref(w),
+                                                                 ctypes.byref(need), ctypes.byref(unused), ctypes.byref(res))
+        self.ctx._check(rc, "decompress_stream_write_host")
+        # (the stream's end lies in this write's input, or in that of writes since the last one that returned
+        # anything but MORE_OUTPUT)
+        self._recent = (self._recent if self.result == MORE_OUTPUT else b"") + bytes(data)
+        self.result, self.needed = res.value, need.value
+        if res.value == SUCCESS:
+            self.eof = True
+            self.unused_data = self._recent[len(self._recent) - unused.value:] if unused.value else b""
+        return res.value, ctypes.string_at(out, w.value), need.value, unused.value
+
+    def _drain(self, data, last, max_length):
+        out = bytearray()
+        if self._buf:       # the rest of a block that did not fit an earlier max_length
+            k = max_length if max_length else len(self._buf)
+            out += self._buf[:k]
+            self._buf = self._buf[k:]
+        while True:
+            room = max_length - len(out) if max_length else max(self._room, 4 * (len(data) + self.pending))
+            res, b, need, _ = self.write(data, last, room)
+            data = b""
+            out += b
+            if res == BAD_DATA:
+                raise Error("decompress stream: bad data")
+            if res != MORE_OUTPUT or (max_length and len(out) >= max_length):
+                break
+            if not max_length:
+                self._room = max(need, 2 * self._room)
+                continue
+            if not b:       # the next block needs more room than is left
+                res, b, _, _ = self.write(b"", last, need)
+                if res == BAD_DATA:
+                    raise Error("decompress stream: bad data")
+                k = max_length - len(out)
+                out += b[:k]
+                self._buf = b[k:]
+                if self._buf or res != MORE_OUTPUT:
+                    break
+        return bytes(out)
+
+    def decompress(self, data, max_length=0):
+        """The output of the complete blocks so far: all of it, or at most max_length bytes (the rest comes from
+        later calls, as with zlib).  Data after the stream's end goes to unused_data."""
+        if self.eof:
+            self.unused_data += bytes(data)
+            return self._drain_buf(max_length)
+        return self._drain(data, False, max_length)
+
+    def _drain_buf(self, max_length):
+        k = max_length if max_length else len(self._buf)
+        out, self._buf = self._buf[:k], self._buf[k:]
+        return out
+
+    def flush(self):
+        """The rest of the output; raises Error when the stream has not ended correctly."""
+        if self.eof:
+            return self._drain_buf(0)
+        return self._drain(b"", True, 0)
+
+    def close(self):
+        if self.h:
+            self.l.libdeflate_b200_decompress_stream_destroy(self.h)
             self.h = None
 
     def __enter__(self):

@@ -58,6 +58,8 @@
 // is extra traffic of the two-kernel split and is reported as such (bench.py "traffic").
 #include "ldb_common.cuh"
 
+#include <vector>
+
 // table geometry
 #define INF_LB        7			// main litlen table bits
 #define INF_LMAIN     (1 << INF_LB)
@@ -321,7 +323,7 @@ __device__ __forceinline__ void inf_warp_copy(u8 *dst, const u8 *src, u32 len, u
 // ---- wrapper headers ------------------------------------------------------------
 // Returns the header size, or 0xffffffff for BAD_DATA.  Sets *footer to the trailer size.
 // ref: lib/gzip_decompress.c:45-98, lib/zlib_decompress.c:45-66
-__device__ u32 inf_parse_wrapper(const u8 *in, size_t n, int format, u32 *footer)
+__host__ __device__ u32 inf_parse_wrapper(const u8 *in, size_t n, int format, u32 *footer)
 {
 	*footer = 0;
 	if (format == LDB_FMT_RAW) return 0;
@@ -360,6 +362,20 @@ __device__ u32 inf_parse_wrapper(const u8 *in, size_t n, int format, u32 *footer
 		if (pos > n || n - pos < 8) return 0xffffffffu;
 	}
 	return (u32)pos;
+}
+
+// The same parser on the host, for a stream whose start arrives in pieces.  Once the fixed part is there, the
+// n bytes are followed by zeros: they end every name and comment and cover every extra field and trailer, so
+// the parse fails only on a bad header, and the header is complete once every byte it spans is one of the n.
+long ldb_stream_wrapper_bytes(const u8 *in, size_t n, int format)
+{
+	if (n < (format == LDB_FMT_GZIP ? 10u : format == LDB_FMT_ZLIB ? 2u : 0u)) return -2;
+	std::vector<u8> b(in, in + n);
+	b.resize(n + 65536 + 64, 0);
+	u32 footer;
+	const u32 hdr = inf_parse_wrapper(b.data(), b.size(), format, &footer);
+	if (hdr == 0xffffffffu) return -1;
+	return hdr <= n ? (long)hdr : -2;
 }
 
 // ---- per-lane header parsing ----------------------------------------------------
@@ -869,6 +885,50 @@ __device__ __forceinline__ bool inf_seg_stop(inf_lane &s, const ldb_seg_args &g,
 	return s.split_i < g.nsplit && g.split[s.split_i] == e;
 }
 
+// Stream form (g.mode != 0), at a block end the lane has reached (a block header, or the end of the last
+// block it decodes): past the open end the lane is STARVED; with the output beyond the room the segment is FULL
+// at the block end recorded before, and 'need' counts through this one; otherwise the open literal run is
+// closed into a record (the resolve then sees exactly the tokens before this point) and the block end is
+// recorded in g.info.  Returns the stop verdict, or 0.
+__device__ __forceinline__ u32 inf_seg_block_end(inf_lane &s, const ldb_inflate_args &a, const ldb_seg_args &g)
+{
+	ldb_seg_info &r = g.info[s.chunk];
+	const u64 P = inf_bits_consumed(s);
+	if ((g.mode & LDB_SEG_OPEN) && P > 8ull * s.in_n) return LDB_SEG_STARVED;
+	const u32 out = inf_out_pos(s) - s.pfx;
+	if (out > a.out_avail[s.chunk]) {
+		r.need = out - r.out_len;
+		return LDB_SEG_FULL;
+	}
+	const bool fits = inf_seg_fits(s, 8);
+	if (fits) inf_flush_pending(s);
+	if (s.n_lit != s.lit_mark) {
+		if (fits) inf_put_record(s, LDB_TOK_PURE_FLAG | (s.n_lit - s.lit_mark));
+		else s.n_rec++;
+		s.lit_mark = s.n_lit;
+	}
+	r.end = 8 * s.seg_base + P;
+	r.out_len = out;
+	r.reach = s.reach;
+	r.n_rec = s.n_rec;
+	r.n_lit = s.n_lit;
+	r.overflow = !fits;
+	return 0;
+}
+
+// Open end, at a block header: does the header, or the stored block it starts, reach past the input?  (The
+// parser would call that BAD_DATA; here it only means that the rest has not arrived.)
+__device__ __forceinline__ bool inf_seg_header_cut(inf_lane &s)
+{
+	const u64 P = inf_bits_consumed(s), n = s.in_n;
+	if (P + 3 > 8 * n) return true;
+	if (((inf_peek(s) >> 1) & 3) != DEFLATE_BLOCKTYPE_STORED) return false;
+	const u64 B = (P + 10) >> 3;	// the stored header after the 3 bits and the padding to a byte
+	if (B + 4 > n) return true;
+	const u32 len = s.in[B] | ((u32)s.in[B + 1] << 8), nlen = s.in[B + 2] | ((u32)s.in[B + 3] << 8);
+	return len == (nlen ^ 0xffffu) && B + 4 + len > n;
+}
+
 template <bool SEG>
 __global__ void __launch_bounds__(32 * INF_WPC, INF_MIN_CTAS)
 ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
@@ -896,7 +956,21 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 			ldb_seg_info r;
 			u32 verdict = s.verdict;
 			const u64 P = inf_bits_consumed(s);
-			r.end = 0; r.trailer = 0; r.isize = 0; r.pad = 0; r.overflow = 0;
+			if (g.mode) {	// the stream form: the last block's end, or a failure that may be the open end
+				const bool open = g.mode & LDB_SEG_OPEN;
+				if (verdict == LDB_SUCCESS && P > 8ull * s.in_n) verdict = open ? LDB_SEG_STARVED : LDB_BAD_DATA;
+				else if (verdict == LDB_SUCCESS || verdict == LDB_SEG_STOPPED) {
+					const u32 v = inf_seg_block_end(s, a, g);
+					verdict = v ? v : verdict;
+				} else if (open && verdict != LDB_SEG_ABANDONED && verdict != LDB_SEG_FULL && P + 64 > 8ull * s.in_n)
+					verdict = LDB_SEG_STARVED;
+				if (verdict == LDB_SEG_STARVED || verdict == LDB_SEG_FULL) {	// the block end recorded last
+					g.info[c].verdict = verdict;
+					s.state = ST_IDLE;
+					return;
+				}
+			}
+			r.end = 0; r.trailer = 0; r.isize = 0; r.need = 0; r.overflow = 0;
 			r.split_j = s.split_i;
 			if (verdict == LDB_SUCCESS) {
 				if (P > (u64)s.in_n * 8) verdict = LDB_BAD_DATA;	// decompress_template.h:754
@@ -1010,6 +1084,11 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 							s.lit_limit = s.out_avail;
 							s.acc = 0;
 							s.pend_len = 0;
+							if (g.mode) {	// the room is checked at block ends; the start is the first one
+								s.out_avail = s.lit_limit = 0xfffffff0u;
+								ldb_seg_info &r = g.info[c];
+								r.end = st; r.out_len = 0; r.reach = 0; r.n_rec = 0; r.n_lit = pfx; r.overflow = 0; r.need = 0;
+							}
 							s.lit = a.tok_base + (a.tok_off[c] - a.tok_origin);
 							s.rec_end = (u32 *)(a.tok_base + (a.tok_off[c + 1] - a.tok_origin));
 							s.cap = a.tok_off[c + 1] - a.tok_off[c];
@@ -1086,9 +1165,20 @@ ldb_inflate_decode_kernel(ldb_inflate_args a, u32 *work_counter, ldb_seg_args g)
 			// one starts there.  At sync points the segment ends after the empty stored block, in (3).)
 			if (s.state == ST_HEADER) {
 				bool stop = false;
-				if constexpr (SEG) stop = g.any_header && inf_seg_stop(s, g, 8 * s.seg_base + inf_bits_consumed(s));
+				u32 stop_v = LDB_SEG_STOPPED;
+				if constexpr (SEG) {
+					if (g.mode) {	// the stream form: every header is a block end
+						stop_v = inf_seg_block_end(s, a, g);
+						if (!stop_v && (g.mode & LDB_SEG_OPEN) && inf_seg_header_cut(s)) stop_v = LDB_SEG_STARVED;
+						stop = stop_v != 0;
+					}
+					if (!stop) {
+						stop_v = LDB_SEG_STOPPED;
+						stop = g.any_header && inf_seg_stop(s, g, 8 * s.seg_base + inf_bits_consumed(s));
+					}
+				}
 				if (stop) {
-					s.verdict = LDB_SEG_STOPPED;
+					s.verdict = stop_v;
 					s.state = ST_DONE;
 				} else {
 					int v = inf_parse_block_header(s, sm, lane, gs_lane + INF_GS_LENS);

@@ -237,20 +237,32 @@ int ldb_launch_verify_trailer(const ldb_inflate_args &a, const u32 *d_checksums,
 // j >= split_i[c] (sync points: only after a non-final empty stored block).  Tokens that do not fit the slot are counted, not written.  With overrun != 0 every
 // chunk but chunk 0 of the launch (whose start is known to be true) gives up once its input passes
 // split[split_i[c]] by more than overrun bits.
+// Stream form (mode != 0, decompress streams, DESIGN.md section 4.8): the wrapper is the caller's (the launch
+// passes RAW), out_avail[c] is the segment's room, checked at every block end, and at every block end the open
+// literal run is closed into a record and the block end is recorded in info[c].  A block whose output passes
+// the room ends the segment at the block end before it (LDB_SEG_FULL, 'need' = the output through the end of
+// that block).  With LDB_SEG_OPEN the input ends at in_nbytes with no trailer after it: a lane that needs a
+// bit past that end, or fails within 8 bytes of it, stops with LDB_SEG_STARVED.  After FULL and STARVED,
+// end, out_len, reach and the token counts describe the last block end passed (the segment start if none).
 #define LDB_SEG_PREFIX 32768u
 struct ldb_seg_info {
-	u64 end;		// stop: the split point's bit offset; final block: the byte offset after its last byte
-	u32 verdict;		// LDB_* result, LDB_SEG_STOPPED or LDB_SEG_ABANDONED
+	u64 end;		// stop: the split point's bit offset; final block: the byte offset after its last byte;
+				// FULL / STARVED: the bit offset of the last block end passed
+	u32 verdict;		// LDB_* result, LDB_SEG_STOPPED, LDB_SEG_ABANDONED, LDB_SEG_STARVED or LDB_SEG_FULL
 	u32 out_len;		// output bytes (the prefix not counted)
 	u32 reach;		// deepest match reach before the segment start (0: none)
 	u32 split_j;		// stop: index of the split point it stopped at
 	u32 n_rec, n_lit;	// token counts (n_lit includes the prefix)
 	u32 overflow;		// the tokens did not fit the slot (counts are exact, contents incomplete)
 	u32 trailer, isize;	// final block: the trailer fields that follow it
-	u32 pad;
+	u32 need;		// FULL: output bytes from 'end' through the end of the block that did not fit
 };
 #define LDB_SEG_STOPPED 16
 #define LDB_SEG_ABANDONED 17
+#define LDB_SEG_STARVED 18
+#define LDB_SEG_FULL 19
+#define LDB_SEG_STREAM 1u	// ldb_seg_args.mode: the stream form
+#define LDB_SEG_OPEN 2u		// ... with an open end
 struct ldb_seg_args {
 	const u8 *base;		// the whole input
 	u64 in_nbytes;
@@ -263,7 +275,11 @@ struct ldb_seg_args {
 	u64 overrun;		// bits a speculative chunk may read past its next split point (0: no limit)
 	u32 any_header;		// split points are found block starts: stop at any header on one (0: sync points,
 				// stop only after a non-final empty stored block that ends on one)
+	u32 mode;		// 0, or LDB_SEG_STREAM with or without LDB_SEG_OPEN
 };
+// A decompress stream's wrapper header from the n bytes of its start: its size, -2 while more bytes are
+// needed, -1 when it is bad (the decode kernel's own parser, inflate_kernel.cu)
+long ldb_stream_wrapper_bytes(const u8 *in, size_t n, int format);
 int ldb_launch_inflate_seg(const ldb_inflate_args &a, const ldb_seg_args &g, const ldb_launch_cfg &cfg, void *stream);
 // resolve of the high byte plane of 16-bit symbols: every chunk reads its literals from 'lit' instead of its slot
 int ldb_launch_inflate_resolve_lit(const ldb_inflate_args &a, const u8 *lit, const ldb_launch_cfg &cfg, void *stream);

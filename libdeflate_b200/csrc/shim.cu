@@ -1583,19 +1583,44 @@ static int li_split_points(libdeflate_b200_ctx *ctx, const u8 *in, size_t n, u64
 
 extern "C" size_t libdeflate_b200_decompress_large_segments(struct libdeflate_b200_ctx *ctx) { return ctx->li_segments; }
 
-extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
-						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
-						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+// One chain of segments over one stream's DEFLATE data (DESIGN.md 4.6, 4.8): decompress_large decodes a whole
+// stream with it, a decompress stream the input it holds.
+struct li_call {
+	int format;		// what the decode kernel parses (a decompress stream passes RAW: its wrapper is parsed on the host)
+	unsigned flags;
+	const u8 *in;
+	size_t n;		// the input the kernel sees (it subtracts the trailer of 'format')
+	u64 data_end;		// where the DEFLATE data ends: split points lie before it
+	u32 footer;		// trailer bytes after the final block (in actual_in)
+	u64 start;		// bit offset of the first block
+	size_t hist;		// output bytes before the start that matches may reach (<= 32 KiB) ...
+	const u8 *window;	// ... right-aligned in these 32 KiB (NULL: the stream start)
+	u32 mode;		// 0, or the stream form (LDB_SEG_STREAM, LDB_SEG_OPEN)
+	u8 *out;
+	size_t room;
+};
+struct li_chain_rec { u64 G, len; };
+struct li_run {
+	ldb_large_verdict v;	// result -1 never leaves; LDB_SEG_STARVED / LDB_SEG_FULL: the chain stopped at 'stop'
+	std::vector<li_chain_rec> chain;
+	u64 stop;		// STARVED / FULL: the bit offset where the undelivered input starts
+	u32 need;		// FULL: output bytes of the block that did not fit
+	u64 out;		// output bytes written
+};
+
+// The chain, its waves, resolves, windows and substitution.  The window after the last chain segment is left in
+// ctx->li_carry.
+static int li_chain(libdeflate_b200_ctx *ctx, const li_call &call, li_run *run)
 {
-	int rc = check_format(format);
-	if (rc) return rc;
-	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
-	ctx->li_segments = 0;
-	const u8 *in = (const u8 *)d_in;
-	u8 *out = (u8 *)d_out;
-	const size_t n = in_nbytes;
-	const u32 footer = ldb_trl_bytes(format);
-	const u64 data_end = n >= footer ? n - footer : 0;	// the DEFLATE data ends before the trailer
+	const int format = call.format;
+	const unsigned flags = call.flags;
+	const u8 *in = call.in;
+	u8 *out = call.out;
+	const size_t n = call.n, out_avail = call.room, hist = call.hist;
+	const u32 footer = call.footer;
+	const u64 data_end = call.data_end;
+	const bool stream = call.mode != 0;
+	int rc;
 
 	// ---- 1. split points: sync points, else found block starts -----------------------------------------
 	std::vector<u64> split;
@@ -1615,12 +1640,13 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	g0.split = (const u64 *)ctx->li_scan.p;
 	g0.nsplit = (u32)split.size();
 	g0.any_header = found;
-	auto seg_start = [&](size_t k) -> u64 { return k ? split[k - 1] : 0; };
+	g0.mode = call.mode;
+	auto seg_start = [&](size_t k) -> u64 { return k ? split[k - 1] : call.start; };
 	auto seg_desc = [&](size_t k, u32 pfx, size_t room) {
 		li_seg_desc d;
 		d.start = seg_start(k);
 		d.pfx = pfx;
-		d.split_i = (u32)(k ? k : 0);
+		d.split_i = (u32)k;
 		d.room = room;
 		const u64 hint_end = k + 1 < nseg ? split[k] : 8 * (u64)n;
 		d.slot = align_up(pfx + ldb_inflate_tok_cap((hint_end - d.start + 7) >> 3, out_avail) + 64, 16);
@@ -1628,10 +1654,13 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	};
 
 	// ---- 2..6. waves of consecutive segments, from the current chain segment on ---------------------
-	struct chain_rec { u64 G, len; };
-	std::vector<chain_rec> chain;
-	ldb_large_verdict v = {};
+	std::vector<li_chain_rec> &chain = run->chain;
+	chain.clear();
+	ldb_large_verdict &v = run->v;
+	v = {};
 	v.result = -1;
+	run->stop = 0;
+	run->need = 0;
 	const u64 budget = token_budget_bytes();
 	// the most segments one wave decodes (the token budget bounds a wave as well)
 	const size_t wave_max = ldb_env_size("LIBDEFLATE_B200_LARGE_WAVE_SEGMENTS", (size_t)1 << 20);
@@ -1643,11 +1672,13 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	size_t cur = 0;		// the next chain segment
 	rc = ldb_reserve_dev(ctx->li_carry, LDB_SEG_PREFIX);
 	if (rc) return rc;
-	LDB_CUDA_CHECK_RET(cudaMemsetAsync(ctx->li_carry.p, 0, LDB_SEG_PREFIX, ctx->stream));
-	// the one segment whose verdict is the stream's, decoded again with its exact room and prefix
+	if (call.window) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_carry.p, call.window, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
+	else LDB_CUDA_CHECK_RET(cudaMemsetAsync(ctx->li_carry.p, 0, LDB_SEG_PREFIX, ctx->stream));
+	// the one segment whose verdict is the stream's, decoded again with its exact room and prefix (the stream
+	// form checks room at block ends, so its verdict is decoded with ample room)
 	auto verdict_of = [&](size_t k) -> int {
-		const u32 pfx = (u32)(G < LDB_SEG_PREFIX ? G : LDB_SEG_PREFIX);
-		li_seg_desc d = seg_desc(k, pfx, out_avail - G);
+		const u32 pfx = (u32)(hist + G < LDB_SEG_PREFIX ? hist + G : LDB_SEG_PREFIX);
+		li_seg_desc d = seg_desc(k, pfx, stream ? (size_t)0xfffffff0u : out_avail - G);
 		d.slot = 0;		// only the verdict is wanted: every token is counted, none written
 		std::vector<li_seg_desc> one(1, d);
 		int rc2 = ldb_reserve_dev(ctx->li_arr, li_layout_bytes(1));
@@ -1659,9 +1690,10 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		ldb_seg_info r;
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(&r, d_info, sizeof(r), cudaMemcpyDeviceToHost, ctx->stream));
 		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
-		if (r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED)
+		if (r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED || r.verdict == LDB_SEG_FULL)
 			return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment decoded alone disagrees with its chain", __FILE__, __LINE__);
 		v.result = (s32)r.verdict;
+		if (r.verdict == LDB_SEG_STARVED) run->stop = seg_start(k);	// the failure may be the open end: nothing of it yet
 		return 0;
 	};
 	while (v.result < 0) {
@@ -1669,7 +1701,8 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		std::vector<li_seg_desc> segs;
 		u64 tok_bytes = 0;
 		for (size_t k = k0; k < nseg && segs.size() < wave_max; k++) {
-			li_seg_desc d = seg_desc(k, k ? LDB_SEG_PREFIX : 0, out_avail);
+			// (the stream form gives every segment of the wave the room after the chain so far: exact for the first)
+			li_seg_desc d = seg_desc(k, k || hist ? LDB_SEG_PREFIX : 0, stream ? out_avail - G : out_avail);
 			if (!segs.empty() && tok_bytes + d.slot > budget) break;
 			segs.push_back(d);
 			tok_bytes += d.slot;
@@ -1700,8 +1733,11 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 			const ldb_seg_info &r = info[j];
 			const size_t k = k0 + j;
 			if (r.verdict == LDB_SEG_ABANDONED) { cur = k; break; }	// the next wave starts with it, uncapped
-			const bool ok = r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED;
-			if (!ok || r.reach > G || r.out_len > out_avail - G) {
+			const bool stop = stream && (r.verdict == LDB_SEG_STARVED || r.verdict == LDB_SEG_FULL);
+			const bool ok = r.verdict == LDB_SUCCESS || r.verdict == LDB_SEG_STOPPED || stop;
+			// (stream form: a later segment of the wave that passes its room starts the next wave, with its room)
+			if (stream && ok && j && r.out_len > out_avail - G) { cur = k; break; }
+			if (!ok || r.reach > hist + G || r.out_len > out_avail - G) {
 				// the segment's own limits: its input and output positions are 32-bit
 				if (data_end - (seg_start(k) >> 3) > 0xfffffff0u && r.verdict != LDB_SEG_STOPPED)
 					return ldb_fail(cudaErrorInvalidValue, "decompress_large: a segment has more than 4 GiB - 16 of input", __FILE__, __LINE__);
@@ -1715,6 +1751,12 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 			wG[j] = G;
 			chain.push_back({G, r.out_len});
 			G += r.out_len;
+			if (stop) {	// the last complete block that fits: the call's chain ends here
+				v.result = (s32)r.verdict;
+				run->stop = r.end;
+				run->need = r.need;
+				break;
+			}
 			if (r.verdict == LDB_SUCCESS) {		// the final block: the stream ends here
 				v.actual_in = r.end + footer;
 				v.actual_out = G;
@@ -1727,7 +1769,8 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 			if (next >= k1) { cur = next; break; }
 			j = next - k0;
 		}
-		if (v.result > 0) break;	// failed (or SHORT_OUTPUT): the output is not contractual
+		// failed (or SHORT_OUTPUT): the output is not contractual
+		if (v.result > 0 && v.result != LDB_SEG_STARVED && v.result != LDB_SEG_FULL) break;
 
 		// ---- re-decode the chain segments whose tokens overflowed their slots, with exact slots ----
 		std::vector<size_t> redo;
@@ -1755,8 +1798,10 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		std::vector<u64> poff(w, 0), plen(w, 0);
 		u64 plane_bytes = 0;
 		u32 max_lit = 0;
+		// (a chain segment with no output before it has no prefix: it is resolved straight into out)
+		auto rel = [&](size_t c) { return k0 + c != 0 || hist != 0; };
 		for (size_t c : wchain) {
-			if (k0 + c == 0) continue;
+			if (!rel(c)) continue;
 			plen[c] = align_up(LDB_SEG_PREFIX + (u64)info[c].out_len + 16, 16);
 			poff[c] = plane_bytes;
 			plane_bytes += (info[c].reach ? 2 : 1) * plen[c];
@@ -1774,8 +1819,8 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 			LDB_CUDA_CHECK_RET(cudaMemcpyAsync((u8 *)ctx->li_hilit.p + 16, pat.data(), LDB_SEG_PREFIX, cudaMemcpyHostToDevice, ctx->stream));
 		}
 		const u8 *hilit = max_lit ? (const u8 *)ctx->li_hilit.p + 16 : nullptr;
-		auto lo_of = [&](size_t c) { return k0 + c ? planes + poff[c] : out + wG[c]; };
-		auto hi_of = [&](size_t c) { return k0 + c && info[c].reach ? planes + poff[c] + plen[c] : nullptr; };
+		auto lo_of = [&](size_t c) { return rel(c) ? planes + poff[c] : out + wG[c]; };
+		auto hi_of = [&](size_t c) { return rel(c) && info[c].reach ? planes + poff[c] + plen[c] : nullptr; };
 
 		// ---- resolve: group 0 = the wave's decode (minus the overflowed), group 1 = the re-decode ----
 		for (int grp = 0; grp < 2; grp++) {
@@ -1793,7 +1838,7 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 				if (on) {
 					lo[i] = lo_of(c);
 					hi[i] = hi_of(c);
-					if (k0 + c) pre.push_back(tok + off);	// the slot's literal stream starts with the prefix
+					if (rel(c)) pre.push_back(tok + off);	// the slot's literal stream starts with the prefix
 				}
 				off += gs[i].slot;
 			}
@@ -1812,11 +1857,10 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		std::vector<ldb_chain_seg> cs(nc);
 		for (size_t m = 0; m < nc; m++) {
 			const size_t c = wchain[m];
-			const bool rel = k0 + c != 0;
-			cs[m].lo = rel ? lo_of(c) + LDB_SEG_PREFIX : out;
+			cs[m].lo = rel(c) ? lo_of(c) + LDB_SEG_PREFIX : out;
 			const u8 *h = hi_of(c);
 			cs[m].hi = h ? h + LDB_SEG_PREFIX : nullptr;
-			cs[m].dst = rel ? out + wG[c] : nullptr;
+			cs[m].dst = rel(c) ? out + wG[c] : nullptr;
 			cs[m].len = info[c].out_len;
 		}
 		rc = ldb_reserve_dev(ctx->li_win, (nc + 1) * (size_t)LDB_SEG_PREFIX);
@@ -1833,24 +1877,61 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
 	}
 	ctx->li_segments = chain.size() ? chain.size() : 1;
+	run->out = G;
+	return 0;
+}
 
-	// ---- 7. checksum of the output, in order, against the trailer; the results ----------------------
-	const size_t nch = v.result == LDB_SUCCESS && format != LDB_FMT_RAW ? chain.size() : 0;
-	rc = ldb_reserve_dev(ctx->li_sums, nch * 20 + 1024);
+// The CRC-32 / Adler-32 of the first nch chain segments' output, one per segment (d_sums), and their lengths
+static int li_chain_sums(libdeflate_b200_ctx *ctx, int format, const u8 *out, const std::vector<li_chain_rec> &chain, size_t nch,
+			 u32 **d_sums, size_t **d_lens)
+{
+	int rc = ldb_reserve_dev(ctx->li_sums, nch * 20 + 1024);
 	if (rc) return rc;
 	u8 *sb = (u8 *)ctx->li_sums.p;
 	const void **d_ptrs = (const void **)sb;
-	size_t *d_lens = (size_t *)(sb + align_up(nch * 8, 256));
-	u32 *d_sums = (u32 *)(sb + 2 * align_up(nch * 8, 256));
-	if (nch) {
-		std::vector<const void *> hp(nch);
-		std::vector<size_t> hl(nch);
-		for (size_t i = 0; i < nch; i++) { hp[i] = out + chain[i].G; hl[i] = chain[i].len; }
-		LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)d_ptrs, hp.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
-		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d_lens, hl.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
-		rc = launch_checksum(ctx, format, d_ptrs, d_lens, d_sums, nch);
-		if (rc) return rc;
-	}
+	*d_lens = (size_t *)(sb + align_up(nch * 8, 256));
+	*d_sums = (u32 *)(sb + 2 * align_up(nch * 8, 256));
+	if (!nch) return 0;
+	std::vector<const void *> hp(nch);
+	std::vector<size_t> hl(nch);
+	for (size_t i = 0; i < nch; i++) { hp[i] = out + chain[i].G; hl[i] = chain[i].len; }
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync((void *)d_ptrs, hp.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(*d_lens, hl.data(), nch * 8, cudaMemcpyHostToDevice, ctx->stream));
+	return launch_checksum(ctx, format, d_ptrs, *d_lens, *d_sums, nch);
+}
+
+extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
+						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+{
+	int rc = check_format(format);
+	if (rc) return rc;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	ctx->li_segments = 0;
+	u8 *out = (u8 *)d_out;
+	const size_t n = in_nbytes;
+	const u32 footer = ldb_trl_bytes(format);
+	li_call call = {};
+	call.format = format;
+	call.flags = flags;
+	call.in = (const u8 *)d_in;
+	call.n = n;
+	call.data_end = n >= footer ? n - footer : 0;	// the DEFLATE data ends before the trailer
+	call.footer = footer;
+	call.out = out;
+	call.room = out_avail;
+	li_run run;
+	rc = li_chain(ctx, call, &run);
+	if (rc) return rc;
+	const ldb_large_verdict &v = run.v;
+	const std::vector<li_chain_rec> &chain = run.chain;
+
+	// ---- 7. checksum of the output, in order, against the trailer; the results ----------------------
+	const size_t nch = v.result == LDB_SUCCESS && format != LDB_FMT_RAW ? chain.size() : 0;
+	u32 *d_sums;
+	size_t *d_lens;
+	rc = li_chain_sums(ctx, format, out, chain, nch, &d_sums, &d_lens);
+	if (rc) return rc;
 	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_inflate_finish(d_sums, d_lens, nch, format, v, d_actual_in, d_actual_out, d_result, ctx->stream); });
 }
 
@@ -1881,6 +1962,233 @@ extern "C" int libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx 
 	if (result) *result = r;
 	if (actual_in) *actual_in = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[0] : 0;
 	if (actual_out) *actual_out = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[1] : 0;
+	return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// one stream read call by call (li_chain in the stream form; DESIGN.md 4.8)
+// ---------------------------------------------------------------------------------
+struct libdeflate_b200_decompress_stream {
+	libdeflate_b200_ctx *ctx;
+	int format;
+	u8 *d_in;		// the input held: [off, off + pend) of a buffer of cap bytes
+	size_t off, pend, cap;
+	u32 bit;		// the first undelivered block starts at this bit of the first byte held
+	u8 *d_win;		// the last <= 32 KiB of output, right-aligned in 32 KiB
+	u64 total;		// output bytes delivered
+	u32 sum;		// their CRC-32 / Adler-32
+	bool header;		// the wrapper header has been parsed
+	bool ended;		// the final block is delivered: the trailer is next
+	bool finished;
+};
+
+extern "C" struct libdeflate_b200_decompress_stream *
+libdeflate_b200_decompress_stream_create(struct libdeflate_b200_ctx *ctx, int format)
+{
+	if (!ctx) {
+		ldb_fail(cudaErrorInvalidValue, "decompress_stream_create: no context", __FILE__, __LINE__);
+		return nullptr;
+	}
+	if (check_format(format)) return nullptr;
+	if (cudaSetDevice(ctx->device) != cudaSuccess) {
+		ldb_fail(cudaGetLastError(), "cudaSetDevice", __FILE__, __LINE__);
+		return nullptr;
+	}
+	u8 *w = nullptr;
+	if (cudaMalloc((void **)&w, LDB_SEG_PREFIX) != cudaSuccess) {
+		ldb_fail(cudaGetLastError(), "cudaMalloc(decompress stream)", __FILE__, __LINE__);
+		return nullptr;
+	}
+	libdeflate_b200_decompress_stream *s = new libdeflate_b200_decompress_stream();
+	s->ctx = ctx;
+	s->format = format;
+	s->d_in = nullptr;
+	s->off = s->pend = s->cap = 0;
+	s->bit = 0;
+	s->d_win = w;
+	s->total = 0;
+	s->sum = format == LDB_FMT_ZLIB ? 1 : 0;
+	s->header = format == LDB_FMT_RAW;
+	s->ended = s->finished = false;
+	return s;
+}
+
+extern "C" void libdeflate_b200_decompress_stream_destroy(struct libdeflate_b200_decompress_stream *s)
+{
+	if (!s) return;
+	cudaSetDevice(s->ctx->device);
+	cudaStreamSynchronize(s->ctx->stream);
+	cudaFree(s->d_in);
+	cudaFree(s->d_win);
+	delete s;
+}
+
+extern "C" size_t libdeflate_b200_decompress_stream_pending(const struct libdeflate_b200_decompress_stream *s)
+{
+	return s ? s->pend : 0;
+}
+
+// The device and host forms: 'in' is read with a copy of kind 'in_kind'; the output goes to d_out (device).
+static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t n, cudaMemcpyKind in_kind, int last,
+		    void *d_out, size_t out_avail, size_t *out_nbytes, size_t *out_needed, size_t *in_unused, int32_t *result)
+{
+	if (!s) return ldb_fail(cudaErrorInvalidValue, "decompress_stream_write: no stream", __FILE__, __LINE__);
+	if (s->finished) return ldb_fail(cudaErrorInvalidValue, "decompress_stream_write: the stream is finished", __FILE__, __LINE__);
+	if (!out_nbytes || !result) return ldb_fail(cudaErrorInvalidValue, "decompress_stream_write: no result", __FILE__, __LINE__);
+	if (n && !in) return ldb_fail(cudaErrorInvalidValue, "decompress_stream_write: no input", __FILE__, __LINE__);
+	if (out_avail && !d_out) return ldb_fail(cudaErrorInvalidValue, "decompress_stream_write: no output", __FILE__, __LINE__);
+	libdeflate_b200_ctx *ctx = s->ctx;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	// ---- the input joins the bytes held (moved to the front of a new buffer when it does not fit) ----
+	if (s->off + s->pend + n > s->cap) {
+		const size_t cap = std::max((size_t)65536, 2 * (s->pend + n));
+		u8 *b = nullptr;
+		LDB_CUDA_CHECK_RET(cudaMalloc((void **)&b, cap));
+		if (s->pend) {
+			cudaError_t e = cudaMemcpyAsync(b, s->d_in + s->off, s->pend, cudaMemcpyDeviceToDevice, ctx->stream);
+			if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+			if (e != cudaSuccess) { cudaFree(b); return ldb_fail(e, "decompress_stream_write: move the input held", __FILE__, __LINE__); }
+		}
+		cudaFree(s->d_in);
+		s->d_in = b;
+		s->off = 0;
+		s->cap = cap;
+	}
+	u8 *held = s->d_in + s->off;
+	if (n) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(held + s->pend, in, n, in_kind, ctx->stream));
+	const size_t have = s->pend + n;
+	size_t used = 0;	// bytes of 'held' the call has consumed
+	u32 bit = s->bit;
+	size_t out_n = 0, need = 0, unused = 0;
+	s32 r = LIBDEFLATE_B200_MORE_INPUT;
+	bool header = s->header, ended = s->ended;
+	u64 total = s->total;
+	u32 sum = s->sum;
+	// ---- the wrapper header, parsed on the host from the first bytes (more of them until it is complete) ----
+	if (!header) {
+		std::vector<u8> h;
+		long hb = -2;
+		for (size_t k = std::min(have, (size_t)4096);; k = std::min(have, 2 * k)) {
+			h.resize(k);
+			int rc = read_back(ctx, h.data(), held, k);
+			if (rc) return rc;
+			hb = ldb_stream_wrapper_bytes(h.data(), k, s->format);
+			if (hb != -2 || k == have) break;
+		}
+		if (hb == -1) r = LDB_BAD_DATA;
+		else if (hb >= 0) { header = true; used = (size_t)hb; }
+	}
+	// ---- the complete blocks that fit, from the first undelivered one -------------------------------
+	const u32 trl = ldb_trl_bytes(s->format);
+	if (header && !ended) {
+		const size_t m = have - used;
+		li_call call = {};
+		call.format = LDB_FMT_RAW;
+		call.in = held + used;
+		// the last write decodes as decompress_large does: the trailer ends the data; before it the end is open
+		call.data_end = last ? (m >= trl ? m - trl : 0) : m;
+		call.n = call.data_end;
+		call.start = bit;
+		call.hist = (size_t)std::min(total, (u64)LDB_SEG_PREFIX);
+		call.window = s->d_win;
+		call.mode = LDB_SEG_STREAM | (last ? 0u : LDB_SEG_OPEN);
+		call.out = (u8 *)d_out;
+		call.room = out_avail;
+		li_run run;
+		int rc = li_chain(ctx, call, &run);
+		if (rc) return rc;
+		// what was written: its checksum, in order, after the one carried; the window after it
+		const size_t nch = s->format != LDB_FMT_RAW ? run.chain.size() : 0;
+		u32 *d_sums;
+		size_t *d_lens;
+		rc = li_chain_sums(ctx, s->format, (const u8 *)d_out, run.chain, nch, &d_sums, &d_lens);
+		if (rc) return rc;
+		std::vector<u32> sums(nch);
+		if (nch) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(sums.data(), d_sums, nch * 4, cudaMemcpyDeviceToHost, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(s->d_win, ctx->li_carry.p, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+		u32 xp[64];
+		xp[0] = 0x00800000u;	// x^8
+		for (int i = 1; i < 64; i++) xp[i] = ldb_mulmodp(xp[i - 1], xp[i - 1]);
+		for (size_t i = 0; i < nch; i++) sum = ldb_sum_combine(s->format, xp, sum, sums[i], run.chain[i].len);
+		out_n = run.out;
+		total += run.out;
+		const s32 v = run.v.result;
+		if (v == LDB_SUCCESS) {			// the final block is delivered; run.v.actual_in is the byte after it
+			ended = true;
+			used += run.v.actual_in;
+			bit = 0;
+		} else if (v == LDB_SEG_STARVED || v == LDB_SEG_FULL) {
+			used += run.stop >> 3;
+			bit = (u32)(run.stop & 7);
+			r = v == LDB_SEG_FULL ? LIBDEFLATE_B200_MORE_OUTPUT : LIBDEFLATE_B200_MORE_INPUT;
+			need = run.need;
+		} else {
+			r = LDB_BAD_DATA;
+		}
+	}
+	// ---- the trailer, once all of it is there ---------------------------------------------------------
+	if (ended) {
+		if (have - used >= trl) {
+			u8 t[8] = {0};
+			int rc = read_back(ctx, t, held + used, trl);
+			if (rc) return rc;
+			bool ok = true;
+			if (s->format == LDB_FMT_GZIP)
+				ok = (t[0] | ((u32)t[1] << 8) | ((u32)t[2] << 16) | ((u32)t[3] << 24)) == sum &&
+				     (t[4] | ((u32)t[5] << 8) | ((u32)t[6] << 16) | ((u32)t[7] << 24)) == (u32)total;
+			else if (s->format == LDB_FMT_ZLIB)
+				ok = (((u32)t[0] << 24) | ((u32)t[1] << 16) | ((u32)t[2] << 8) | t[3]) == sum;
+			used += trl;
+			unused = have - used;
+			r = ok ? LDB_SUCCESS : LDB_BAD_DATA;
+		} else {
+			r = LIBDEFLATE_B200_MORE_INPUT;
+		}
+	}
+	if (last && r == LIBDEFLATE_B200_MORE_INPUT) r = LDB_BAD_DATA;	// every complete block is delivered, the stream has not ended
+	// ---- commit -------------------------------------------------------------------------------------------
+	s->off += used;
+	s->pend = have - used;
+	s->bit = bit;
+	s->header = header;
+	s->ended = ended;
+	s->total = total;
+	s->sum = sum;
+	s->finished = r == LDB_SUCCESS || r == LDB_BAD_DATA;
+	if (s->finished) s->pend = 0;
+	*out_nbytes = out_n;
+	if (out_needed) *out_needed = r == LIBDEFLATE_B200_MORE_OUTPUT ? need : 0;
+	if (in_unused) *in_unused = r == LDB_SUCCESS ? unused : 0;
+	*result = r;
+	return 0;
+}
+
+extern "C" int libdeflate_b200_decompress_stream_write(struct libdeflate_b200_decompress_stream *s, const void *d_in, size_t in_nbytes,
+							int last, void *d_out, size_t out_avail, size_t *out_nbytes,
+							size_t *out_needed, size_t *in_unused, int32_t *result)
+{
+	return ds_write(s, d_in, in_nbytes, cudaMemcpyDeviceToDevice, last, d_out, out_avail, out_nbytes, out_needed, in_unused, result);
+}
+
+extern "C" int libdeflate_b200_decompress_stream_write_host(struct libdeflate_b200_decompress_stream *s, const void *in, size_t in_nbytes,
+							     int last, void *out, size_t out_avail, size_t *out_nbytes,
+							     size_t *out_needed, size_t *in_unused, int32_t *result)
+{
+	if (!s) return ldb_fail(cudaErrorInvalidValue, "decompress_stream_write_host: no stream", __FILE__, __LINE__);
+	libdeflate_b200_ctx *ctx = s->ctx;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	stream_quiesce quiesce(ctx);
+	// (the device sees the caller's 16-byte output phase)
+	u8 *d_out;
+	int rc = stage_one(ctx, ctx->d_stage_out, out, out_avail, false, &d_out);
+	if (rc) return rc;
+	size_t w = 0;
+	rc = ds_write(s, in, in_nbytes, cudaMemcpyHostToDevice, last, d_out, out_avail, &w, out_needed, in_unused, result);
+	if (rc) return rc;
+	rc = read_back(ctx, out, d_out, w);
+	if (rc) return rc;
+	if (out_nbytes) *out_nbytes = w;
 	return 0;
 }
 

@@ -3,14 +3,19 @@
 A minimal gzip-style front end over the blocked-gzip (BGZF) calls, standing in for the part of the
 reference's programs/gzip.c that drives the library (compress: programs/gzip.c:170-174, decompress loop:
 :249-273).  Compressed files are ordinary multi-member .gz files (readable by any gunzip); decompression
-accepts blocked gzip files (ours, bgzip's).  There is no CPU fallback: without a CUDA device this fails.
+accepts blocked gzip files (ours, bgzip's) and any other gzip file, which it reads in READ_SIZE pieces through
+decompress streams, so that memory does not grow with the file.  There is no CPU fallback: without a CUDA device
+this fails.
 """
 import argparse
+import itertools
 import os
 import struct
 import sys
 
 import libdeflate_b200 as ldb
+
+READ_SIZE = 64 << 20    # bytes per read of a file that is not blocked gzip
 
 
 def uncompressed_size(data):
@@ -97,6 +102,33 @@ def decompress_members_large(ctx, data):
     return b"".join(out)
 
 
+def decompress_stream(ctx, pieces, write):
+    """Any multi-member gzip file, given as successive pieces of bytes: one decompress stream per member, the
+    next one started from the bytes after the member's end (unused_data).  Each member is decoded by the whole
+    GPU as its input arrives; write() receives the output as it is produced, and only the input after the last
+    complete block is held."""
+    d, members = None, 0
+    try:
+        for piece in pieces:
+            while piece:
+                if d is None:
+                    d = ctx.decompressobj(ldb.GZIP)
+                write(d.decompress(piece))
+                piece = b""
+                if d.eof:
+                    piece = d.unused_data
+                    d.close()
+                    d, members = None, members + 1
+        if d is not None:
+            write(d.flush())
+            members += 1
+    except ldb.Error as e:
+        raise ValueError("decompression failed in member %d: %s" % (members, e))
+    finally:
+        if d is not None:
+            d.close()
+
+
 def main(argv=None, ctx=None, api=None):
     ap = argparse.ArgumentParser(prog="python -m libdeflate_b200.gz", description=__doc__.split("\n\n")[1])
     ap.add_argument("-d", "--decompress", action="store_true")
@@ -109,14 +141,34 @@ def main(argv=None, ctx=None, api=None):
     level = 6 if args.level is None else args.level
     ctx = ctx or ldb.Context(0)
     for path in args.files:
-        data = open(path, "rb").read()
         if args.decompress:
-            try:
-                out = decompress_bytes(ctx, data)
-            except ValueError:
-                out = decompress_members_large(ctx, data)     # not blocked: member by member
             dst = path[:-3] if path.endswith(".gz") else path + ".out"
+            with open(path, "rb") as f:
+                head = f.read(READ_SIZE)
+                if len(head) > 3 and head[:3] == b"\x1f\x8b\x08" and head[3] & 4:    # may be blocked gzip
+                    data = head + f.read()
+                    try:
+                        out = [decompress_bytes(ctx, data)]
+                    except ValueError:
+                        out = None
+                    pieces = [data]
+                else:
+                    out = None
+                    pieces = itertools.chain([head], iter(lambda: f.read(READ_SIZE), b""))
+                sink = sys.stdout.buffer if args.stdout else open(dst, "wb")
+                try:
+                    if out is not None:
+                        sink.write(out[0])
+                    else:       # not blocked: member by member, as the file is read
+                        decompress_stream(ctx, pieces, sink.write)
+                finally:
+                    if not args.stdout:
+                        sink.close()
+            if not args.stdout and not args.keep:
+                os.remove(path)
+            continue
         else:
+            data = open(path, "rb").read()
             out = compress_bytes(ctx, data, level)
             dst = path + ".gz"
         if args.stdout:
