@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["shim.cu", "checksum_kernels.cu", "inflate_kernel.cu", "inflate_resolve.cu", "deflate_kernel.cu", "pack_kernels.cu", "large_kernels.cu", "large_inflate.cu"]
-HEADERS = ["ldb_common.cuh", "deflate_lz_kernel.cuh", "deflate_block.cuh"]
+HEADERS = ["ldb_common.cuh", "deflate_lz_kernel.cuh", "deflate_block.cuh", "deflate_parse.cuh"]
 LIB = os.path.join(HERE, "libdeflate_b200.so")
 EMU_DIR = os.path.join(ROOT, "tests", "emu")
 EMU_LIB = os.path.join(EMU_DIR, "_build", "libdeflate_b200_emu.so")

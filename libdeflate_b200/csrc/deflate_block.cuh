@@ -5,15 +5,23 @@
 // the LZ_SM_* layout; the flush scratch aliases the parse region R, never live at the same time.
 #pragma once
 
-// The threads [0, gt) (warps [0, gw)) that flush a block; sync() is their barrier.
+// A group of gw warps (gt threads) that runs one stage: the calling thread's rank tid, lane and warp in it,
+// and sync(), its barrier: named barrier 'bar' for a group smaller than the CTA, __syncthreads for the CTA.
 struct lz_group {
-	u32 tid, lane, warp, gw, gt;
+	u32 tid, lane, warp, gw, gt, bar;
 	__device__ __forceinline__ void sync() const
 	{
-		if (gt < LZ_THREADS) LDB_BAR_SYNC(LZ_BAR_P, gt);
+		if (gt < LZ_THREADS) LDB_BAR_SYNC(bar, gt);
 		else __syncthreads();
 	}
 };
+
+// The group of the nw warps from warp w0 on, with barrier 'bar', as seen by one of its threads.
+__device__ __forceinline__ lz_group lz_group_of(u32 w0, u32 nw, u32 bar)
+{
+	const u32 tid = threadIdx.x - 32 * w0;
+	return {tid, tid & 31, tid >> 5, nw, 32 * nw, bar};
+}
 
 // precode code lengths in the order of the dynamic header (RFC 1951 3.2.7)
 __constant__ u8 lz_precode_perm[DEFLATE_NUM_PRECODE_SYMS] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
