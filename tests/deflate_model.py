@@ -17,6 +17,9 @@ check_stream() disassembles a whole stream and asserts, for every block, that wh
 what the model makes of the block's own histograms, plus the stream's structural rules: distances, block
 extents, BFINAL, and for pieces of compress_large / compress_stream the closing empty stored block and the
 dictionary reach.
+
+The tokens themselves are the LZ stage's: tests/lz_model.py models that stage, and with this model writes the
+exact stream, which tests/test_deflate_lz_model.py compares with the kernel's.
 """
 import zlib
 
