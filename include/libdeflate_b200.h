@@ -403,6 +403,74 @@ libdeflate_b200_decompress_stream_write_host(struct libdeflate_b200_decompress_s
 					     const void *in, size_t in_nbytes, int last, void *out, size_t out_avail,
 					     size_t *out_nbytes, size_t *out_needed, size_t *in_unused, int32_t *result);
 
+/*
+ * An INDEX of one large DEFLATE / zlib / gzip stream: built once by a full decode, it lets any byte ranges
+ * of the stream's output be read without decoding what comes before them (zlib's zran.c, indexed_gzip).
+ *
+ * Access points: the decode of decompress_large proves a chain of segment starts; the index keeps a subset.
+ *   Point 0 is the first DEFLATE bit after the wrapper, at output 0; after it, the first chain start whose
+ *   output offset is at least 'spacing' past the previous point and at least 32 KiB.  A point records its
+ *   input bit, its output offset, the CRC-32 of its span (the output up to the next point) and the 32 KiB of
+ *   output before it (device memory).  A stream that decompress_large decodes as one segment gets one point,
+ *   and every extract from it is a one-lane decode of the whole stream.  gzip: the first member only.
+ *
+ * index_build: decodes exactly as decompress_large does (same bytes in d_out; *result, *actual_in and
+ *   *actual_out, host values here, are decompress_large's) and WAITS for the trailer check.  On SUCCESS
+ *   *index is a new index of the stream, otherwise NULL.  spacing 0 = LIBDEFLATE_B200_INDEX_SPACING; at most
+ *   1 GiB.  index_build_host: host buffers, staging included.
+ * An index belongs to the context it was built or loaded on and is destroyed before it.
+ * index_serialize: the index as a blob of index_serialized_size bytes (little-endian: header, point table,
+ *   windows, CRC-32 of everything before it; DESIGN.md section 4.9), independent of the context.
+ * index_load: the index of a blob; NULL (last_error() says why) when the blob is malformed: a wrong magic,
+ *   version, format or point kind, sizes that do not add up exactly, access points whose bits or output
+ *   offsets are not strictly increasing, lie out of range or (after point 0) before 32 KiB, or a bad CRC.
+ *
+ * index_extract: range i is output bytes [h_offsets[i], h_offsets[i] + h_lens[i]) of the indexed stream,
+ *   written to d_dst[i] (a host array of device pointers); h_results[i] (host) is LIBDEFLATE_SUCCESS, or
+ *   LIBDEFLATE_BAD_DATA when a span it needs does not decode from its point to the next one (or, the last, to
+ *   the stream's end) with the recorded length and CRC-32 (d_in is not the indexed stream, or the index is
+ *   not its index).  A BAD_DATA range's bytes are undefined, but nothing is written outside
+ *   [d_dst[i], d_dst[i] + h_lens[i]), and the input is never written.  Each span a call needs is decoded
+ *   once, all of them at once, from the point's window.  The decode reads only the input from the byte of
+ *   the first needed point to the end of the last needed span, plus LIBDEFLATE_B200_INDEX_READ_MARGIN bytes.
+ *   It returns an error code, having done nothing, when a range passes index_out_nbytes or in_nbytes is not
+ *   the indexed stream's.  It WAITS, as decompress_large does.
+ * index_extract_host: host input and destinations; only the input bytes the decode reads are staged.
+ * Kernel time: decode as kind 2, resolve as kind 5, span CRCs as kind 0, the copies (windows, prefixes,
+ * ranges) as kind 6; index_build adds the kinds of decompress_large.
+ */
+#define LIBDEFLATE_B200_INDEX_SPACING      262144    /* default spacing: output bytes between access points */
+#define LIBDEFLATE_B200_INDEX_READ_MARGIN  16        /* input bytes an extract's decode may read past its last span */
+struct libdeflate_b200_index;
+LIBDEFLATEAPI int
+libdeflate_b200_index_build(struct libdeflate_b200_ctx *ctx, int format, unsigned flags, const void *d_in, size_t in_nbytes,
+			    void *d_out, size_t out_avail, size_t spacing, size_t *actual_in, size_t *actual_out,
+			    int32_t *result, struct libdeflate_b200_index **index);
+LIBDEFLATEAPI int
+libdeflate_b200_index_build_host(struct libdeflate_b200_ctx *ctx, int format, unsigned flags, const void *in, size_t in_nbytes,
+				 void *out, size_t out_avail, size_t spacing, size_t *actual_in, size_t *actual_out,
+				 int32_t *result, struct libdeflate_b200_index **index);
+LIBDEFLATEAPI void
+libdeflate_b200_index_destroy(struct libdeflate_b200_index *ix);
+LIBDEFLATEAPI size_t
+libdeflate_b200_index_points(const struct libdeflate_b200_index *ix);
+LIBDEFLATEAPI uint64_t
+libdeflate_b200_index_out_nbytes(const struct libdeflate_b200_index *ix);
+LIBDEFLATEAPI size_t
+libdeflate_b200_index_serialized_size(const struct libdeflate_b200_index *ix);
+LIBDEFLATEAPI int
+libdeflate_b200_index_serialize(const struct libdeflate_b200_index *ix, void *buf, size_t avail);
+LIBDEFLATEAPI struct libdeflate_b200_index *
+libdeflate_b200_index_load(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes);
+LIBDEFLATEAPI int
+libdeflate_b200_index_extract(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *d_in,
+			      size_t in_nbytes, const uint64_t *h_offsets, const size_t *h_lens, void *const *d_dst,
+			      int32_t *h_results, size_t n_ranges);
+LIBDEFLATEAPI int
+libdeflate_b200_index_extract_host(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *in,
+				   size_t in_nbytes, const uint64_t *h_offsets, const size_t *h_lens, void *const *h_dst,
+				   int32_t *h_results, size_t n_ranges);
+
 #ifdef __cplusplus
 }
 #endif

@@ -56,8 +56,14 @@ BATCH_SYMBOLS = [
     "libdeflate_b200_decompress_stream_create", "libdeflate_b200_decompress_stream_destroy",
     "libdeflate_b200_decompress_stream_pending", "libdeflate_b200_decompress_stream_write",
     "libdeflate_b200_decompress_stream_write_host",
+    "libdeflate_b200_index_build", "libdeflate_b200_index_build_host", "libdeflate_b200_index_destroy",
+    "libdeflate_b200_index_points", "libdeflate_b200_index_out_nbytes", "libdeflate_b200_index_serialized_size",
+    "libdeflate_b200_index_serialize", "libdeflate_b200_index_load", "libdeflate_b200_index_extract",
+    "libdeflate_b200_index_extract_host",
 ]
 LARGE_PIECE = 131072    # LIBDEFLATE_B200_LARGE_PIECE: input bytes per piece of compress_large
+INDEX_SPACING = 262144      # LIBDEFLATE_B200_INDEX_SPACING: default output bytes between access points
+INDEX_READ_MARGIN = 16      # LIBDEFLATE_B200_INDEX_READ_MARGIN: input an extract may read past its last span
 NO_FLUSH, SYNC_FLUSH, FINISH = 0, 1, 2     # flush modes of a compress stream's write
 SUCCESS, BAD_DATA = 0, 1                   # libdeflate results
 MORE_INPUT, MORE_OUTPUT = 0x100, 0x101     # the other results of a decompress stream's write
@@ -201,6 +207,26 @@ def load_library(path=None):
         fn = getattr(lib, "libdeflate_b200_decompress_stream_" + f)
         fn.restype = c_int
         fn.argtypes = [P, P, S, c_int, P, S, PS, PS, PS, POINTER(c_int32)]
+    for f in ("build", "build_host"):
+        fn = getattr(lib, "libdeflate_b200_index_" + f)
+        fn.restype = c_int
+        fn.argtypes = [P, c_int, c_uint, P, S, P, S, S, PS, PS, POINTER(c_int32), POINTER(P)]
+    lib.libdeflate_b200_index_destroy.restype = None
+    lib.libdeflate_b200_index_destroy.argtypes = [P]
+    lib.libdeflate_b200_index_points.restype = S
+    lib.libdeflate_b200_index_points.argtypes = [P]
+    lib.libdeflate_b200_index_out_nbytes.restype = c_uint64
+    lib.libdeflate_b200_index_out_nbytes.argtypes = [P]
+    lib.libdeflate_b200_index_serialized_size.restype = S
+    lib.libdeflate_b200_index_serialized_size.argtypes = [P]
+    lib.libdeflate_b200_index_serialize.restype = c_int
+    lib.libdeflate_b200_index_serialize.argtypes = [P, P, S]
+    lib.libdeflate_b200_index_load.restype = P
+    lib.libdeflate_b200_index_load.argtypes = [P, P, S]
+    for f in ("extract", "extract_host"):
+        fn = getattr(lib, "libdeflate_b200_index_" + f)
+        fn.restype = c_int
+        fn.argtypes = [P, P, P, S, P, P, P, P, S]
     return lib
 
 
@@ -449,6 +475,27 @@ class Context:
             return res.value, None, 0, 0
         return SUCCESS, ctypes.string_at(out, aout.value), ain.value, aout.value
 
+    def decompress_large_index(self, data, out_avail, fmt=RAW, spacing=0):
+        """decompress_large's tuple (result, bytes or None, actual_in, actual_out) plus an Index of the stream
+        (None unless the result is SUCCESS).  spacing: output bytes between access points (0: INDEX_SPACING)."""
+        addr, n, keep = _buf_ptr(data)
+        out = ctypes.create_string_buffer(max(out_avail, 1))
+        ain, aout, res, ix = c_size_t(0), c_size_t(0), c_int32(0), c_void_p(None)
+        self._check(self.l.libdeflate_b200_index_build_host(
+            self.h, fmt, 0, addr, n, out, out_avail, spacing, ctypes.byref(ain), ctypes.byref(aout), ctypes.byref(res),
+            ctypes.byref(ix)), "index_build_host")
+        if res.value != SUCCESS:
+            return res.value, None, 0, 0, None
+        return SUCCESS, ctypes.string_at(out, aout.value), ain.value, aout.value, Index(self, ix.value)
+
+    def load_index(self, blob):
+        """The Index of a serialized blob (Index.to_bytes()); raises Error when the blob is malformed."""
+        addr, n, keep = _buf_ptr(blob)
+        h = self.l.libdeflate_b200_index_load(self.h, addr, n)
+        if not h:
+            raise Error("index_load failed: %s" % self.l.libdeflate_b200_last_error().decode())
+        return Index(self, h)
+
     def compressobj(self, level=6, fmt=RAW):
         """A CompressStream on this context: ONE stream written call by call, like zlib.compressobj."""
         return CompressStream(self, level, fmt)
@@ -534,6 +581,55 @@ class Context:
         finally:
             for p in (d_data, d_ptrs, d_sizes, d_vals):
                 self.l.libdeflate_b200_device_free(self.h, p)
+
+
+class Index:
+    """libdeflate_b200_index: access points into one stream, from which any byte ranges of its output decode
+    without what comes before them (Context.decompress_large_index, Context.load_index)."""
+
+    def __init__(self, ctx, h):
+        self.ctx = ctx
+        self.l = ctx.l
+        self.h = h
+        ctx._streams.add(self)
+
+    @property
+    def points(self):
+        return self.l.libdeflate_b200_index_points(self.h)
+
+    @property
+    def out_nbytes(self):
+        return self.l.libdeflate_b200_index_out_nbytes(self.h)
+
+    def to_bytes(self):
+        n = self.l.libdeflate_b200_index_serialized_size(self.h)
+        buf = ctypes.create_string_buffer(n)
+        self.ctx._check(self.l.libdeflate_b200_index_serialize(self.h, buf, n), "index_serialize")
+        return buf.raw
+
+    def read(self, data, ranges):
+        """[(result, bytes or None)] for each (offset, length) of 'ranges', from the indexed stream 'data' (host)."""
+        addr, n, keep = _buf_ptr(data)
+        k = len(ranges)
+        offs = (c_uint64 * max(k, 1))(*[o for o, _ in ranges])
+        lens = (c_size_t * max(k, 1))(*[ln for _, ln in ranges])
+        bufs = [ctypes.create_string_buffer(max(ln, 1)) for _, ln in ranges]
+        dst = (c_void_p * max(k, 1))(*[ctypes.addressof(b) for b in bufs])
+        res = (c_int32 * max(k, 1))()
+        self.ctx._check(self.l.libdeflate_b200_index_extract_host(self.ctx.h, self.h, addr, n, offs, lens, dst, res, k),
+                        "index_extract_host")
+        return [(res[i], bufs[i].raw[:ranges[i][1]] if res[i] == SUCCESS else None) for i in range(k)]
+
+    def close(self):
+        if self.h:
+            self.l.libdeflate_b200_index_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class CompressStream:

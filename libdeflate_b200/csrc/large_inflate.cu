@@ -390,6 +390,53 @@ int ldb_launch_substitute(const ldb_chain_seg *d_segs, size_t n, const u8 *d_win
 	return 0;
 }
 
+// ---- piece copies of the index (DESIGN.md section 4.9) ------------------------------------------------
+// One kernel for the three copies of an index: the windows of new access points out of the chain's window
+// array (index_build), the real window bytes into a span's literal prefix, and the ranges' pieces out of the
+// staged spans (index_extract).  CTA b copies pieces b, b + grid, ...; a piece is head bytes up to a 16-byte
+// aligned destination, then 16-byte rows when source and destination share their phase, else aligned words
+// built from the two aligned source words that hold them (an aligned load never leaves the allocation that
+// holds one of its bytes), then tail bytes.
+#define LI_COPY_THREADS 256
+__global__ void __launch_bounds__(LI_COPY_THREADS)
+ldb_copy_pieces_kernel(const ldb_copy_piece *pieces, size_t n)
+{
+	for (size_t j = blockIdx.x; j < n; j += gridDim.x) {
+		const ldb_copy_piece pc = pieces[j];
+		const u8 *src = pc.src;
+		u8 *dst = pc.dst;
+		const u64 mis = (16 - ((uintptr_t)dst & 15)) & 15;
+		const u64 head = mis < pc.len ? mis : pc.len;
+		for (u64 i = threadIdx.x; i < head; i += LI_COPY_THREADS) dst[i] = src[i];
+		src += head;
+		dst += head;
+		const u64 len = pc.len - head;
+		u64 body;
+		if ((((uintptr_t)src ^ (uintptr_t)dst) & 15) == 0) {
+			body = len & ~(u64)15;
+			for (u64 i = threadIdx.x; i < body / 16; i += LI_COPY_THREADS) ((uint4 *)dst)[i] = ((const uint4 *)src)[i];
+		} else {
+			body = len & ~(u64)3;
+			const u32 sh = 8 * (u32)((uintptr_t)src & 3);
+			const u32 *s4 = (const u32 *)((uintptr_t)src & ~(uintptr_t)3);
+			for (u64 i = threadIdx.x; i < body / 4; i += LI_COPY_THREADS) {
+				const u64 w = sh ? ((u64)s4[i + 1] << 32 | s4[i]) >> sh : (u64)s4[i];
+				((u32 *)dst)[i] = (u32)w;
+			}
+		}
+		for (u64 i = body + threadIdx.x; i < len; i += LI_COPY_THREADS) dst[i] = src[i];
+	}
+}
+
+int ldb_launch_copy_pieces(const ldb_copy_piece *d_pieces, size_t n, void *stream)
+{
+	if (!n) return 0;
+	const size_t blocks = n < 65535 ? n : 65535;
+	LDB_LAUNCH(ldb_copy_pieces_kernel, dim3((unsigned)blocks), dim3(LI_COPY_THREADS), 0, (cudaStream_t)stream, d_pieces, n);
+	LDB_CUDA_CHECK_RET(cudaGetLastError());
+	return 0;
+}
+
 // ---- finish: ordered checksum combine, trailer check, results (one CTA) -------------------------------
 #define LI_FIN_THREADS 1024
 __global__ void __launch_bounds__(LI_FIN_THREADS)

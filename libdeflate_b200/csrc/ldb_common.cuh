@@ -298,6 +298,12 @@ int ldb_launch_block_scan(const u8 *in, size_t n, u64 *d_count, u64 *d_cand, u64
 int ldb_launch_seg_prefix_fill(u8 *const *d_lit, size_t n, void *stream);
 int ldb_launch_window_chain(const ldb_chain_seg *d_segs, size_t n, u8 *d_windows, void *stream);
 int ldb_launch_substitute(const ldb_chain_seg *d_segs, size_t n, const u8 *d_windows, void *stream);
+struct ldb_copy_piece {		// one copy of the index's piece-copy kernel (DESIGN.md section 4.9)
+	const u8 *src;
+	u8 *dst;
+	u64 len;
+};
+int ldb_launch_copy_pieces(const ldb_copy_piece *d_pieces, size_t n, void *stream);
 struct ldb_large_verdict {
 	s32 result;		// decided on the host; SUCCESS may still turn into BAD_DATA at the trailer check
 	u32 trailer, isize;

@@ -109,6 +109,7 @@ struct libdeflate_b200_ctx {
 	// decompress_large (device): sync-point scan + split list, per-wave arrays, re-decoded tokens,
 	// symbol planes, windows, the carried window, the high-plane literal stream, checksum arrays
 	ldb_buf li_scan, li_arr, li_tok2, li_planes, li_win, li_carry, li_hilit, li_sums;
+	ldb_buf li_copy;		// device: piece lists of the index's copy kernel
 	size_t li_segments;		// chain segments of the last decompress_large
 	ldb_buf d_params;		// device: pointer/size arrays for host-buffer calls
 	ldb_buf h_pinned;		// pinned host staging
@@ -235,7 +236,7 @@ extern "C" void libdeflate_b200_ctx_destroy(struct libdeflate_b200_ctx *ctx)
 	cudaFree(ctx->d_pack.p);
 	cudaFree(ctx->large.p);
 	cudaFree(ctx->cs_stage.p);
-	for (ldb_buf *b : {&ctx->li_scan, &ctx->li_arr, &ctx->li_tok2, &ctx->li_planes, &ctx->li_win, &ctx->li_carry, &ctx->li_hilit, &ctx->li_sums})
+	for (ldb_buf *b : {&ctx->li_scan, &ctx->li_arr, &ctx->li_tok2, &ctx->li_planes, &ctx->li_win, &ctx->li_carry, &ctx->li_hilit, &ctx->li_sums, &ctx->li_copy})
 		cudaFree(b->p);
 	cudaFree(ctx->d_params.p);
 	if (ctx->h_pinned.p) cudaFreeHost(ctx->h_pinned.p);
@@ -1585,6 +1586,7 @@ extern "C" size_t libdeflate_b200_decompress_large_segments(struct libdeflate_b2
 
 // One chain of segments over one stream's DEFLATE data (DESIGN.md 4.6, 4.8): decompress_large decodes a whole
 // stream with it, a decompress stream the input it holds.
+struct li_index_sink;
 struct li_call {
 	int format;		// what the decode kernel parses (a decompress stream passes RAW: its wrapper is parsed on the host)
 	unsigned flags;
@@ -1598,8 +1600,9 @@ struct li_call {
 	u32 mode;		// 0, or the stream form (LDB_SEG_STREAM, LDB_SEG_OPEN)
 	u8 *out;
 	size_t room;
+	li_index_sink *index;	// NULL, or where index_build collects access points and their windows
 };
-struct li_chain_rec { u64 G, len; };
+struct li_chain_rec { u64 G, len, start; };	// start: the segment's first bit in the input
 struct li_run {
 	ldb_large_verdict v;	// result -1 never leaves; LDB_SEG_STARVED / LDB_SEG_FULL: the chain stopped at 'stop'
 	std::vector<li_chain_rec> chain;
@@ -1607,6 +1610,62 @@ struct li_run {
 	u32 need;		// FULL: output bytes of the block that did not fit
 	u64 out;		// output bytes written
 };
+
+// ---- the index's access points, collected wave by wave (DESIGN.md 4.9) ----------------------------------
+// Point 0 is the first DEFLATE bit at output 0 (the caller fills its bit).  A chain segment's start becomes the
+// next point when its G is at least 'spacing' past the previous point and at least 32 KiB: its window is then
+// the full W_k, which the wave's window chain has just written and the next wave overwrites.
+struct li_index_sink {
+	u64 spacing;
+	std::vector<u64> bit, out;	// the points
+	bool any_header = false;	// they are found block starts (ldb_seg_args.any_header)
+	u8 *d_win = nullptr;		// the windows of points 1, 2, ... (32 KiB each); owned by the sink until taken
+	size_t win_cap = 0;		// windows d_win holds room for
+	~li_index_sink() { cudaFree(d_win); }
+};
+
+// Copies a list of pieces with the copy kernel; the list goes through ctx->li_copy (a later list waits for the
+// copy before it: both are on the context's stream).
+static int li_copy(libdeflate_b200_ctx *ctx, const std::vector<ldb_copy_piece> &pc)
+{
+	if (pc.empty()) return 0;
+	int rc = ldb_reserve_dev(ctx->li_copy, pc.size() * sizeof(ldb_copy_piece) + 256);
+	if (rc) return rc;
+	ldb_copy_piece *d = (ldb_copy_piece *)ctx->li_copy.p;
+	LDB_CUDA_CHECK_RET(cudaMemcpyAsync(d, pc.data(), pc.size() * sizeof(ldb_copy_piece), cudaMemcpyHostToDevice, ctx->stream));
+	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_copy_pieces(d, pc.size(), ctx->stream); });
+}
+
+// One wave's chain segments recs[0, nc), whose windows W before each are at win + m x 32 KiB
+static int li_index_take(libdeflate_b200_ctx *ctx, li_index_sink &ix, const li_chain_rec *recs, size_t nc, const u8 *win)
+{
+	std::vector<size_t> take;
+	for (size_t m = 0; m < nc; m++)
+		if (recs[m].G >= LDB_SEG_PREFIX && recs[m].G - ix.out.back() >= ix.spacing) {
+			ix.bit.push_back(recs[m].start);
+			ix.out.push_back(recs[m].G);
+			take.push_back(m);
+		}
+	if (take.empty()) return 0;
+	const size_t nw = ix.out.size() - 1;
+	if (nw > ix.win_cap) {		// grown by doubling, the windows so far kept
+		const size_t cap = std::max(nw, 2 * ix.win_cap);
+		u8 *w = nullptr;
+		LDB_CUDA_CHECK_RET(cudaMalloc((void **)&w, cap * (size_t)LDB_SEG_PREFIX));
+		if (ix.win_cap) {
+			cudaError_t e = cudaMemcpyAsync(w, ix.d_win, (nw - take.size()) * (size_t)LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream);
+			if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+			if (e != cudaSuccess) { cudaFree(w); return ldb_fail(e, "index_build: grow the windows", __FILE__, __LINE__); }
+		}
+		cudaFree(ix.d_win);
+		ix.d_win = w;
+		ix.win_cap = cap;
+	}
+	std::vector<ldb_copy_piece> pc;
+	for (size_t i = 0; i < take.size(); i++)
+		pc.push_back({win + take[i] * (size_t)LDB_SEG_PREFIX, ix.d_win + (nw - take.size() + i) * (size_t)LDB_SEG_PREFIX, LDB_SEG_PREFIX});
+	return li_copy(ctx, pc);
+}
 
 // The chain, its waves, resolves, windows and substitution.  The window after the last chain segment is left in
 // ctx->li_carry.
@@ -1641,6 +1700,7 @@ static int li_chain(libdeflate_b200_ctx *ctx, const li_call &call, li_run *run)
 	g0.nsplit = (u32)split.size();
 	g0.any_header = found;
 	g0.mode = call.mode;
+	if (call.index) call.index->any_header = found;
 	auto seg_start = [&](size_t k) -> u64 { return k ? split[k - 1] : call.start; };
 	auto seg_desc = [&](size_t k, u32 pfx, size_t room) {
 		li_seg_desc d;
@@ -1749,7 +1809,7 @@ static int li_chain(libdeflate_b200_ctx *ctx, const li_call &call, li_run *run)
 			}
 			wchain.push_back(j);
 			wG[j] = G;
-			chain.push_back({G, r.out_len});
+			chain.push_back({G, r.out_len, seg_start(k)});
 			G += r.out_len;
 			if (stop) {	// the last complete block that fits: the call's chain ends here
 				v.result = (s32)r.verdict;
@@ -1871,6 +1931,7 @@ static int li_chain(libdeflate_b200_ctx *ctx, const li_call &call, li_run *run)
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(win, ctx->li_carry.p, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
 		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_window_chain((const ldb_chain_seg *)d_cs, nc, win, ctx->stream); });
 		if (!rc) rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_substitute((const ldb_chain_seg *)d_cs, nc, win, ctx->stream); });
+		if (!rc && call.index) rc = li_index_take(ctx, *call.index, chain.data() + chain.size() - nc, nc, win);
 		if (rc) return rc;
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_carry.p, win + nc * (size_t)LDB_SEG_PREFIX, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
 		// (the next wave reuses these buffers)
@@ -1900,9 +1961,9 @@ static int li_chain_sums(libdeflate_b200_ctx *ctx, int format, const u8 *out, co
 	return launch_checksum(ctx, format, d_ptrs, *d_lens, *d_sums, nch);
 }
 
-extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
-						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
-						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+// decompress_large, and index_build with an index sink
+static int li_large(libdeflate_b200_ctx *ctx, int format, unsigned flags, const void *d_in, size_t in_nbytes, void *d_out,
+		    size_t out_avail, size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result, li_index_sink *index)
 {
 	int rc = check_format(format);
 	if (rc) return rc;
@@ -1920,6 +1981,7 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	call.footer = footer;
 	call.out = out;
 	call.room = out_avail;
+	call.index = index;
 	li_run run;
 	rc = li_chain(ctx, call, &run);
 	if (rc) return rc;
@@ -1933,6 +1995,13 @@ extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx,
 	rc = li_chain_sums(ctx, format, out, chain, nch, &d_sums, &d_lens);
 	if (rc) return rc;
 	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_large_inflate_finish(d_sums, d_lens, nch, format, v, d_actual_in, d_actual_out, d_result, ctx->stream); });
+}
+
+extern "C" int libdeflate_b200_decompress_large(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
+						 const void *d_in, size_t in_nbytes, void *d_out, size_t out_avail,
+						 size_t *d_actual_in, size_t *d_actual_out, int32_t *d_result)
+{
+	return li_large(ctx, format, flags, d_in, in_nbytes, d_out, out_avail, d_actual_in, d_actual_out, d_result, nullptr);
 }
 
 extern "C" int libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx *ctx, int format, unsigned flags,
@@ -1962,6 +2031,506 @@ extern "C" int libdeflate_b200_decompress_large_host(struct libdeflate_b200_ctx 
 	if (result) *result = r;
 	if (actual_in) *actual_in = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[0] : 0;
 	if (actual_out) *actual_out = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[1] : 0;
+	return 0;
+}
+
+// The wrapper header of the stream whose first 'have' bytes are at d_in (device), parsed on the host from as
+// few of them as it needs: ldb_stream_wrapper_bytes' answer in *hb
+static int wrapper_bytes(libdeflate_b200_ctx *ctx, const u8 *d_in, size_t have, int format, long *hb)
+{
+	std::vector<u8> h;
+	for (size_t k = std::min(have, (size_t)4096);; k = std::min(have, 2 * k)) {
+		h.resize(k);
+		int rc = read_back(ctx, h.data(), d_in, k);
+		if (rc) return rc;
+		*hb = ldb_stream_wrapper_bytes(h.data(), k, format);
+		if (*hb != -2 || k == have) return 0;
+	}
+}
+
+// ---------------------------------------------------------------------------------
+// an index of one stream: access points, then any byte ranges of it (DESIGN.md 4.9)
+// ---------------------------------------------------------------------------------
+#define LI_INDEX_MAGIC 0x5844494cu		// "LIDX"
+#define LI_INDEX_VERSION 1u
+#define LI_INDEX_HEADER 56			// magic, version, format, any_header, in_nbytes, actual_in, out_nbytes, spacing, points
+#define LI_INDEX_POINT 24			// bit, out, crc, 0
+#define LI_INDEX_SPACING_MAX ((size_t)1 << 30)
+#define LI_STAGE_MAX ((u64)1 << 30)		// staged spans per extract wave (one span may pass it alone)
+
+struct libdeflate_b200_index {
+	libdeflate_b200_ctx *ctx;
+	int format;
+	u32 any_header;		// the points are found block starts (ldb_seg_args.any_header), not sync points
+	u64 in_nbytes, actual_in, out_nbytes, spacing;
+	std::vector<u64> bit, out;	// per point: its first input bit, its output offset
+	std::vector<u32> crc;		// per point: the CRC-32 of its span, [out[p], out[p + 1] or out_nbytes)
+	u8 *d_win;			// windows of points 1, 2, ...: 32 KiB each (device)
+};
+
+static u32 h_crc32(const u8 *p, size_t n)
+{
+	static const std::vector<u32> t = [] {
+		std::vector<u32> v(256);
+		for (u32 b = 0; b < 256; b++) {
+			u32 c = b;
+			for (int k = 0; k < 8; k++) c = (c >> 1) ^ (c & 1 ? LDB_CRC32_POLY : 0);
+			v[b] = c;
+		}
+		return v;
+	}();
+	u32 c = 0xffffffffu;
+	for (size_t i = 0; i < n; i++) c = t[(c ^ p[i]) & 255] ^ (c >> 8);
+	return ~c;
+}
+
+static void put64(u8 *p, u64 v) { for (int i = 0; i < 8; i++) p[i] = (u8)(v >> (8 * i)); }
+static u64 get64(const u8 *p) { u64 v = 0; for (int i = 7; i >= 0; i--) v = (v << 8) | p[i]; return v; }
+static void put32(u8 *p, u32 v) { for (int i = 0; i < 4; i++) p[i] = (u8)(v >> (8 * i)); }
+static u32 get32(const u8 *p) { return p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16) | ((u32)p[3] << 24); }
+
+static libdeflate_b200_index *index_new(libdeflate_b200_ctx *ctx)
+{
+	libdeflate_b200_index *ix = new libdeflate_b200_index();
+	ix->ctx = ctx;
+	ix->d_win = nullptr;
+	return ix;
+}
+
+extern "C" void libdeflate_b200_index_destroy(struct libdeflate_b200_index *ix)
+{
+	if (!ix) return;
+	cudaSetDevice(ix->ctx->device);
+	cudaStreamSynchronize(ix->ctx->stream);
+	cudaFree(ix->d_win);
+	delete ix;
+}
+
+extern "C" size_t libdeflate_b200_index_points(const struct libdeflate_b200_index *ix) { return ix ? ix->bit.size() : 0; }
+extern "C" uint64_t libdeflate_b200_index_out_nbytes(const struct libdeflate_b200_index *ix) { return ix ? ix->out_nbytes : 0; }
+
+extern "C" int libdeflate_b200_index_build(struct libdeflate_b200_ctx *ctx, int format, unsigned flags, const void *d_in,
+					   size_t in_nbytes, void *d_out, size_t out_avail, size_t spacing, size_t *actual_in,
+					   size_t *actual_out, int32_t *result, struct libdeflate_b200_index **index)
+{
+	if (!index || !result) return ldb_fail(cudaErrorInvalidValue, "index_build: no result", __FILE__, __LINE__);
+	*index = nullptr;
+	if (spacing > LI_INDEX_SPACING_MAX) return ldb_fail(cudaErrorInvalidValue, "index_build: spacing above 1 GiB", __FILE__, __LINE__);
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	li_index_sink sink;
+	sink.spacing = spacing ? spacing : LIBDEFLATE_B200_INDEX_SPACING;
+	sink.bit.push_back(0);
+	sink.out.push_back(0);
+	int rc = ldb_reserve_dev(ctx->d_params, 256);
+	if (rc) return rc;
+	size_t *d_res = (size_t *)ctx->d_params.p;	// actual_in, actual_out, result
+	LDB_CUDA_CHECK_RET(cudaMemsetAsync(d_res, 0, 3 * sizeof(size_t), ctx->stream));
+	rc = li_large(ctx, format, flags, d_in, in_nbytes, d_out, out_avail, d_res, d_res + 1, (int32_t *)(d_res + 2), &sink);
+	if (rc) return rc;
+	size_t h[3];
+	rc = read_back(ctx, h, d_res, sizeof(h));
+	if (rc) return rc;
+	const int32_t r = (int32_t)h[2];
+	*result = r;
+	if (actual_in) *actual_in = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[0] : 0;
+	if (actual_out) *actual_out = r == LDB_SUCCESS || r == LDB_SHORT_OUTPUT ? h[1] : 0;
+	if (r != LDB_SUCCESS) return 0;
+	// point 0: the first DEFLATE bit; every span's CRC-32 in one batch
+	long hb;
+	rc = wrapper_bytes(ctx, (const u8 *)d_in, in_nbytes, format, &hb);
+	if (rc) return rc;
+	if (hb < 0) return ldb_fail(cudaErrorInvalidValue, "index_build: the wrapper parse disagrees with the decode", __FILE__, __LINE__);
+	sink.bit[0] = 8 * (u64)hb;
+	const size_t np = sink.out.size();
+	std::vector<li_chain_rec> spans(np);
+	for (size_t p = 0; p < np; p++) spans[p] = {sink.out[p], (p + 1 < np ? sink.out[p + 1] : h[1]) - sink.out[p], 0};
+	u32 *d_sums;
+	size_t *d_lens;
+	rc = li_chain_sums(ctx, LDB_FMT_GZIP, (const u8 *)d_out, spans, np, &d_sums, &d_lens);
+	if (rc) return rc;
+	libdeflate_b200_index *ix = index_new(ctx);
+	ix->crc.resize(np);
+	rc = read_back(ctx, ix->crc.data(), d_sums, np * 4);
+	if (rc) { delete ix; return rc; }
+	ix->format = format;
+	ix->any_header = sink.any_header;
+	ix->in_nbytes = in_nbytes;
+	ix->actual_in = h[0];
+	ix->out_nbytes = h[1];
+	ix->spacing = sink.spacing;
+	ix->bit = sink.bit;
+	ix->out = sink.out;
+	ix->d_win = sink.d_win;
+	sink.d_win = nullptr;
+	*index = ix;
+	return 0;
+}
+
+extern "C" int libdeflate_b200_index_build_host(struct libdeflate_b200_ctx *ctx, int format, unsigned flags, const void *in,
+						size_t in_nbytes, void *out, size_t out_avail, size_t spacing, size_t *actual_in,
+						size_t *actual_out, int32_t *result, struct libdeflate_b200_index **index)
+{
+	if (!index || !result) return ldb_fail(cudaErrorInvalidValue, "index_build_host: no result", __FILE__, __LINE__);
+	*index = nullptr;
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	stream_quiesce quiesce(ctx);
+	u8 *d_in, *d_out;
+	int rc = stage_one(ctx, ctx->d_stage_in, in, in_nbytes, true, &d_in);
+	if (!rc) rc = stage_one(ctx, ctx->d_stage_out, out, out_avail, false, &d_out);
+	if (rc) return rc;
+	size_t ain = 0, aout = 0;
+	rc = libdeflate_b200_index_build(ctx, format, flags, d_in, in_nbytes, d_out, out_avail, spacing, &ain, &aout, result, index);
+	if (!rc && *result == LDB_SUCCESS) rc = read_back(ctx, out, d_out, aout);
+	if (rc) {
+		libdeflate_b200_index_destroy(*index);
+		*index = nullptr;
+		return rc;
+	}
+	if (actual_in) *actual_in = ain;
+	if (actual_out) *actual_out = aout;
+	return 0;
+}
+
+// ---- serialized form (little-endian): header, point table, windows, CRC-32 of everything before it ----
+static size_t index_blob_bytes(u64 np) { return LI_INDEX_HEADER + LI_INDEX_POINT * np + (size_t)LDB_SEG_PREFIX * (np - 1) + 4; }
+
+extern "C" size_t libdeflate_b200_index_serialized_size(const struct libdeflate_b200_index *ix)
+{
+	return ix ? index_blob_bytes(ix->bit.size()) : 0;
+}
+
+extern "C" int libdeflate_b200_index_serialize(const struct libdeflate_b200_index *ix, void *buf, size_t avail)
+{
+	if (!ix || !buf) return ldb_fail(cudaErrorInvalidValue, "index_serialize: no index or buffer", __FILE__, __LINE__);
+	const size_t np = ix->bit.size(), total = index_blob_bytes(np);
+	if (avail < total) return ldb_fail(cudaErrorInvalidValue, "index_serialize: the buffer is smaller than index_serialized_size", __FILE__, __LINE__);
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ix->ctx->device));
+	u8 *b = (u8 *)buf;
+	put32(b, LI_INDEX_MAGIC);
+	put32(b + 4, LI_INDEX_VERSION);
+	put32(b + 8, (u32)ix->format);
+	put32(b + 12, ix->any_header);
+	put64(b + 16, ix->in_nbytes);
+	put64(b + 24, ix->actual_in);
+	put64(b + 32, ix->out_nbytes);
+	put64(b + 40, ix->spacing);
+	put64(b + 48, np);
+	u8 *t = b + LI_INDEX_HEADER;
+	for (size_t p = 0; p < np; p++, t += LI_INDEX_POINT) {
+		put64(t, ix->bit[p]);
+		put64(t + 8, ix->out[p]);
+		put32(t + 16, ix->crc[p]);
+		put32(t + 20, 0);
+	}
+	int rc = read_back(ix->ctx, t, ix->d_win, (np - 1) * (size_t)LDB_SEG_PREFIX);
+	if (rc) return rc;
+	put32(b + total - 4, h_crc32(b, total - 4));
+	return 0;
+}
+
+extern "C" struct libdeflate_b200_index *libdeflate_b200_index_load(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes)
+{
+	auto bad = [](const char *why) -> libdeflate_b200_index * { ldb_fail(cudaErrorInvalidValue, why, __FILE__, __LINE__); return nullptr; };
+	if (!ctx || (!buf && nbytes)) return bad("index_load: no context or buffer");
+	const u8 *b = (const u8 *)buf;
+	if (nbytes < LI_INDEX_HEADER + LI_INDEX_POINT + 4) return bad("index_load: shorter than an index");
+	if (get32(b) != LI_INDEX_MAGIC) return bad("index_load: not an index (magic)");
+	if (get32(b + 4) != LI_INDEX_VERSION) return bad("index_load: unknown version");
+	const u32 format = get32(b + 8), any = get32(b + 12);
+	const u64 in_nbytes = get64(b + 16), actual_in = get64(b + 24), out_nbytes = get64(b + 32), spacing = get64(b + 40), np = get64(b + 48);
+	if (format > LDB_FMT_GZIP || any > 1) return bad("index_load: bad format or point kind");
+	if (np == 0 || np > nbytes / LDB_SEG_PREFIX + 1 || index_blob_bytes(np) != nbytes) return bad("index_load: sizes do not add up");
+	if (h_crc32(b, nbytes - 4) != get32(b + nbytes - 4)) return bad("index_load: bad CRC");
+	const u32 trl = ldb_trl_bytes((int)format);
+	if (spacing == 0 || spacing > LI_INDEX_SPACING_MAX || actual_in > in_nbytes || actual_in < trl + 1)
+		return bad("index_load: bad stream sizes");
+	const u64 data_end = actual_in - trl;
+	libdeflate_b200_index *ix = index_new(ctx);
+	ix->format = (int)format;
+	ix->any_header = any;
+	ix->in_nbytes = in_nbytes;
+	ix->actual_in = actual_in;
+	ix->out_nbytes = out_nbytes;
+	ix->spacing = spacing;
+	const u8 *t = b + LI_INDEX_HEADER;
+	for (u64 p = 0; p < np; p++, t += LI_INDEX_POINT) {
+		const u64 bit = get64(t), out = get64(t + 8);
+		const bool ok = get32(t + 20) == 0 && bit < 8 * data_end &&
+				(p == 0 ? out == 0 : bit > ix->bit.back() && out > ix->out.back() && out >= LDB_SEG_PREFIX && out < out_nbytes);
+		if (!ok) { delete ix; return bad("index_load: bad access point"); }
+		ix->bit.push_back(bit);
+		ix->out.push_back(out);
+		ix->crc.push_back(get32(t + 16));
+	}
+	const size_t wb = (size_t)(np - 1) * LDB_SEG_PREFIX;
+	cudaError_t e = cudaSetDevice(ctx->device);
+	if (e == cudaSuccess && wb) e = cudaMalloc((void **)&ix->d_win, wb);
+	if (e == cudaSuccess && wb) e = cudaMemcpy(ix->d_win, t, wb, cudaMemcpyHostToDevice);
+	if (e != cudaSuccess) {
+		ldb_fail(e, "index_load: windows to the device", __FILE__, __LINE__);
+		libdeflate_b200_index_destroy(ix);
+		return nullptr;
+	}
+	return ix;
+}
+
+// ---- extract ------------------------------------------------------------------------------------------
+// The spans the ranges need, in order, and the input bytes [lo, hi) their decode reads: from the byte of the
+// first needed point to the end of the last needed span plus LIBDEFLATE_B200_INDEX_READ_MARGIN
+struct li_plan {
+	std::vector<u32> spans;
+	u64 lo = 0, hi = 0;
+};
+static u64 span_len(const libdeflate_b200_index *ix, size_t p) { return (p + 1 < ix->out.size() ? ix->out[p + 1] : ix->out_nbytes) - ix->out[p]; }
+static u64 span_end_bit(const libdeflate_b200_index *ix, size_t p)
+{
+	return p + 1 < ix->bit.size() ? ix->bit[p + 1] : 8 * (ix->actual_in - ldb_trl_bytes(ix->format));
+}
+static size_t span_of(const libdeflate_b200_index *ix, u64 x) { return (size_t)(std::upper_bound(ix->out.begin(), ix->out.end(), x) - ix->out.begin()) - 1; }
+
+static int li_plan_of(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix, size_t in_nbytes, const uint64_t *offsets,
+		      const size_t *lens, size_t n, li_plan *pl)
+{
+	if (!ix || ix->ctx != ctx) return ldb_fail(cudaErrorInvalidValue, "index_extract: no index, or an index of another context", __FILE__, __LINE__);
+	if (in_nbytes != ix->in_nbytes) return ldb_fail(cudaErrorInvalidValue, "index_extract: in_nbytes differs from the index's", __FILE__, __LINE__);
+	if (n && (!offsets || !lens)) return ldb_fail(cudaErrorInvalidValue, "index_extract: no ranges", __FILE__, __LINE__);
+	std::vector<u8> need(ix->bit.size(), 0);
+	for (size_t i = 0; i < n; i++) {
+		if (offsets[i] > ix->out_nbytes || lens[i] > ix->out_nbytes - offsets[i])
+			return ldb_fail(cudaErrorInvalidValue, "index_extract: a range passes the end of the stream", __FILE__, __LINE__);
+		if (!lens[i]) continue;
+		for (size_t p = span_of(ix, offsets[i]), p1 = span_of(ix, offsets[i] + lens[i] - 1); p <= p1; p++) need[p] = 1;
+	}
+	for (size_t p = 0; p < need.size(); p++)
+		if (need[p]) pl->spans.push_back((u32)p);
+	if (!pl->spans.empty()) {
+		pl->lo = ix->bit[pl->spans.front()] >> 3;
+		pl->hi = std::min(ix->actual_in - ldb_trl_bytes(ix->format), ((span_end_bit(ix, pl->spans.back()) + 7) >> 3) + LIBDEFLATE_B200_INDEX_READ_MARGIN);
+	}
+	return 0;
+}
+
+// 'in' holds the stream's bytes [pl.lo, pl.hi) (device); range i goes to d_dst[i] (device)
+static int li_extract(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix, const li_plan &pl, const u8 *in,
+		      const uint64_t *offsets, const size_t *lens, void *const *d_dst, int32_t *results, size_t n)
+{
+	const size_t np = ix->bit.size();
+	std::vector<u8> ok(np, 0);		// needed spans that decoded and checked
+	int rc;
+	if (!pl.spans.empty()) {
+		// the split list: the points after the first needed one, rebased to 'in'
+		const u32 p0 = pl.spans.front();
+		std::vector<u64> split;
+		for (size_t q = p0 + 1; q < np; q++) split.push_back(ix->bit[q] - 8 * pl.lo);
+		rc = ldb_reserve_dev(ctx->li_scan, split.size() * 8 + 256);
+		if (rc) return rc;
+		if (!split.empty()) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_scan.p, split.data(), split.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+		ldb_seg_args g0 = {};
+		g0.base = in;
+		g0.in_nbytes = pl.hi - pl.lo;
+		g0.split = (const u64 *)ctx->li_scan.p;
+		g0.nsplit = (u32)split.size();
+		g0.any_header = ix->any_header;
+		const u64 budget = token_budget_bytes();
+		std::vector<int> slot_of(np, -1);	// wave-local index of a span of the current wave
+		for (size_t s0 = 0; s0 < pl.spans.size();) {
+			// ---- one wave: spans that fit the token budget and the staging bound ----
+			std::vector<li_seg_desc> segs;
+			std::vector<u32> wp;		// the wave's spans
+			std::vector<u64> soff;		// their staging offsets
+			u64 tok_bytes = 0, stage_bytes = 0;
+			size_t s1 = s0;
+			for (; s1 < pl.spans.size(); s1++) {
+				const u32 p = pl.spans[s1];
+				const u64 len = span_len(ix, p), ib = (span_end_bit(ix, p) - ix->bit[p] + 7) >> 3;
+				const u32 pfx = p ? LDB_SEG_PREFIX : 0;
+				if (len > 0xfffffff0u - LDB_SEG_PREFIX || ib > 0xfffffff0u) continue;	// past the decoder's limits: BAD_DATA
+				li_seg_desc d;
+				d.start = ix->bit[p] - 8 * pl.lo;
+				d.pfx = pfx;
+				d.split_i = p - p0;	// the index of point p + 1 in the split list
+				d.room = len;
+				d.slot = align_up(pfx + ldb_inflate_tok_cap(ib, len) + 64, 16);
+				const u64 sb = align_up(pfx + len + 16, 16);
+				if (!segs.empty() && (tok_bytes + d.slot > budget || stage_bytes + sb > LI_STAGE_MAX)) break;
+				segs.push_back(d);
+				wp.push_back(p);
+				soff.push_back(stage_bytes);
+				tok_bytes += d.slot;
+				stage_bytes += sb;
+			}
+			s0 = s1;
+			const size_t w = segs.size();
+			if (!w) continue;
+			const size_t lay = li_layout_bytes(w), rlay = li_resolve_bytes(w);
+			rc = ldb_reserve_dev(ctx->token_scratch, tok_bytes + 256);
+			if (!rc) rc = ldb_reserve_dev(ctx->li_arr, 2 * lay + 2 * rlay + 256);
+			if (!rc) rc = ldb_reserve_dev(ctx->li_planes, stage_bytes + 256);
+			if (rc) return rc;
+			u8 *arr = (u8 *)ctx->li_arr.p, *stage = (u8 *)ctx->li_planes.p;
+			// ---- 1. decode every span at once (RAW, from its point to the next) ----
+			ldb_inflate_args a;
+			ldb_seg_info *d_info;
+			rc = li_decode(ctx, LDB_FMT_RAW, g0, segs, arr, (u8 *)ctx->token_scratch.p, &a, &d_info);
+			if (rc) return rc;
+			std::vector<ldb_seg_info> info(w);
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(info.data(), d_info, w * sizeof(ldb_seg_info), cudaMemcpyDeviceToHost, ctx->stream));
+			LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+			// a span decodes right when it stops at the next point (or, the last, ends the stream where the index
+			// says), with the recorded length and no match before its window
+			std::vector<u8> good(w);
+			for (size_t i = 0; i < w; i++) {
+				const ldb_seg_info &r = info[i];
+				const u32 p = wp[i];
+				const bool last = p + 1 == np;
+				const bool stop = last ? r.verdict == LDB_SUCCESS && r.end + pl.lo == ix->actual_in - ldb_trl_bytes(ix->format)
+						       : r.verdict == LDB_SEG_STOPPED && r.split_j == segs[i].split_i;
+				good[i] = stop && r.out_len == segs[i].room && r.reach <= segs[i].pfx;
+			}
+			// ---- 2. the spans whose tokens overflowed their slots, decoded again with exact slots ----
+			std::vector<size_t> redo;
+			std::vector<li_seg_desc> rs;
+			u64 bytes = 0;
+			for (size_t i = 0; i < w; i++)
+				if (good[i] && info[i].overflow) {
+					li_seg_desc d = segs[i];
+					d.slot = align_up((u64)info[i].n_lit + 4ull * info[i].n_rec + 64, 16);
+					bytes += d.slot;
+					redo.push_back(i);
+					rs.push_back(d);
+				}
+			ldb_inflate_args a2 = {};
+			if (!redo.empty()) {
+				rc = ldb_reserve_dev(ctx->li_tok2, bytes + 256);
+				if (rc) return rc;
+				ldb_seg_info *d_info2;
+				rc = li_decode(ctx, LDB_FMT_RAW, g0, rs, arr + lay, (u8 *)ctx->li_tok2.p, &a2, &d_info2);
+				if (rc) return rc;
+			}
+			// ---- 3. the literal prefixes take the real windows; 4. resolve: window + span, one byte plane ----
+			std::vector<ldb_copy_piece> pre;
+			for (int grp = 0; grp < 2; grp++) {
+				const std::vector<li_seg_desc> &gs = grp ? rs : segs;
+				u8 *tok = grp ? (u8 *)ctx->li_tok2.p : (u8 *)ctx->token_scratch.p;
+				u64 off = 0;
+				for (size_t j = 0; j < gs.size(); j++) {
+					const size_t i = grp ? redo[j] : j;
+					if (good[i] && (grp || !info[i].overflow) && wp[i])
+						pre.push_back({ix->d_win + (size_t)(wp[i] - 1) * LDB_SEG_PREFIX, tok + off, LDB_SEG_PREFIX});
+					off += gs[j].slot;
+				}
+			}
+			rc = li_copy(ctx, pre);
+			if (rc) return rc;
+			for (int grp = 0; grp < 2; grp++) {
+				const size_t gw = grp ? rs.size() : w;
+				if (!gw) continue;
+				std::vector<ldb_seg_info> ginfo(gw);
+				std::vector<u8 *> lo(gw, nullptr), hi(gw, nullptr);
+				for (size_t j = 0; j < gw; j++) {
+					const size_t i = grp ? redo[j] : j;
+					ginfo[j] = info[i];
+					if (good[i] && (grp || !info[i].overflow)) lo[j] = stage + soff[i];
+				}
+				rc = li_resolve(ctx, grp ? a2 : a, ginfo, lo, hi, nullptr, arr + 2 * lay + grp * rlay);
+				if (rc) return rc;
+			}
+			// ---- 5. the CRC-32 of every staged span against the recorded one ----
+			std::vector<li_chain_rec> cr;
+			std::vector<size_t> ci;
+			for (size_t i = 0; i < w; i++)
+				if (good[i]) {
+					cr.push_back({soff[i] + segs[i].pfx, segs[i].room, 0});
+					ci.push_back(i);
+				}
+			u32 *d_sums;
+			size_t *d_lens;
+			rc = li_chain_sums(ctx, LDB_FMT_GZIP, stage, cr, cr.size(), &d_sums, &d_lens);
+			if (rc) return rc;
+			std::vector<u32> sums(cr.size());
+			rc = read_back(ctx, sums.data(), d_sums, cr.size() * 4);
+			if (rc) return rc;
+			for (size_t m = 0; m < ci.size(); m++) {
+				const size_t i = ci[m];
+				if (sums[m] == ix->crc[wp[i]]) {
+					ok[wp[i]] = 1;
+					slot_of[wp[i]] = (int)i;
+				}
+			}
+			// ---- 6. every range's pieces in the good spans of the wave, in pieces of at most 64 KiB ----
+			std::vector<ldb_copy_piece> pc;
+			for (size_t k = 0; k < n; k++) {
+				if (!lens[k]) continue;
+				const u64 a0 = offsets[k], a1 = offsets[k] + lens[k];
+				for (size_t p = span_of(ix, a0), p1 = span_of(ix, a1 - 1); p <= p1; p++) {
+					if (slot_of[p] < 0) continue;
+					const size_t i = (size_t)slot_of[p];
+					const u64 b0 = std::max(a0, ix->out[p]), b1 = std::min(a1, ix->out[p] + segs[i].room);
+					const u8 *src = stage + soff[i] + segs[i].pfx + (b0 - ix->out[p]);
+					u8 *dst = (u8 *)d_dst[k] + (b0 - a0);
+					for (u64 o = 0; o < b1 - b0; o += 65536) pc.push_back({src + o, dst + o, std::min((u64)65536, b1 - b0 - o)});
+				}
+			}
+			rc = li_copy(ctx, pc);
+			if (rc) return rc;
+			LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));	// (the next wave reuses the staging)
+			for (u32 p : wp) slot_of[p] = -1;
+		}
+	}
+	for (size_t k = 0; k < n; k++) {
+		bool good = true;
+		if (lens[k])
+			for (size_t p = span_of(ix, offsets[k]), p1 = span_of(ix, offsets[k] + lens[k] - 1); p <= p1; p++) good = good && ok[p];
+		results[k] = good ? LDB_SUCCESS : LDB_BAD_DATA;
+	}
+	return 0;
+}
+
+extern "C" int libdeflate_b200_index_extract(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *d_in,
+					     size_t in_nbytes, const uint64_t *h_offsets, const size_t *h_lens, void *const *d_dst,
+					     int32_t *h_results, size_t n_ranges)
+{
+	if (!ctx) return ldb_fail(cudaErrorInvalidValue, "index_extract: no context", __FILE__, __LINE__);
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	li_plan pl;
+	int rc = li_plan_of(ctx, ix, in_nbytes, h_offsets, h_lens, n_ranges, &pl);
+	if (rc) return rc;
+	if (n_ranges && (!d_dst || !h_results)) return ldb_fail(cudaErrorInvalidValue, "index_extract: no destinations or results", __FILE__, __LINE__);
+	return li_extract(ctx, ix, pl, (const u8 *)d_in + pl.lo, h_offsets, h_lens, d_dst, h_results, n_ranges);
+}
+
+extern "C" int libdeflate_b200_index_extract_host(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *in,
+						  size_t in_nbytes, const uint64_t *h_offsets, const size_t *h_lens, void *const *h_dst,
+						  int32_t *h_results, size_t n_ranges)
+{
+	if (!ctx) return ldb_fail(cudaErrorInvalidValue, "index_extract_host: no context", __FILE__, __LINE__);
+	LDB_CUDA_CHECK_RET(cudaSetDevice(ctx->device));
+	li_plan pl;
+	int rc = li_plan_of(ctx, ix, in_nbytes, h_offsets, h_lens, n_ranges, &pl);
+	if (rc) return rc;
+	if (n_ranges && (!h_dst || !h_results)) return ldb_fail(cudaErrorInvalidValue, "index_extract_host: no destinations or results", __FILE__, __LINE__);
+	stream_quiesce quiesce(ctx);
+	// only the compressed bytes the decode reads, and the ranges at their host alignment phases
+	std::vector<size_t> doff(n_ranges);
+	size_t total = 0;
+	for (size_t k = 0; k < n_ranges; k++) {
+		total = align_up(total, 16) + ((uintptr_t)h_dst[k] & 15);
+		doff[k] = total;
+		total += h_lens[k];
+	}
+	u8 *d_in, *d_out;
+	rc = stage_one(ctx, ctx->d_stage_in, (const u8 *)in + pl.lo, pl.hi - pl.lo, true, &d_in);
+	if (!rc) rc = ldb_reserve_dev(ctx->d_stage_out, total + 64);
+	if (rc) return rc;
+	d_out = (u8 *)ctx->d_stage_out.p;
+	std::vector<void *> dd(n_ranges);
+	for (size_t k = 0; k < n_ranges; k++) dd[k] = d_out + doff[k];
+	rc = li_extract(ctx, ix, pl, d_in, h_offsets, h_lens, dd.data(), h_results, n_ranges);
+	if (rc) return rc;
+	for (size_t k = 0; k < n_ranges; k++)
+		if (h_results[k] == LDB_SUCCESS && h_lens[k])
+			LDB_CUDA_CHECK_RET(cudaMemcpyAsync(h_dst[k], dd[k], h_lens[k], cudaMemcpyDeviceToHost, ctx->stream));
+	LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
 	return 0;
 }
 
@@ -2066,15 +2635,9 @@ static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t
 	u32 sum = s->sum;
 	// ---- the wrapper header, parsed on the host from the first bytes (more of them until it is complete) ----
 	if (!header) {
-		std::vector<u8> h;
-		long hb = -2;
-		for (size_t k = std::min(have, (size_t)4096);; k = std::min(have, 2 * k)) {
-			h.resize(k);
-			int rc = read_back(ctx, h.data(), held, k);
-			if (rc) return rc;
-			hb = ldb_stream_wrapper_bytes(h.data(), k, s->format);
-			if (hb != -2 || k == have) break;
-		}
+		long hb;
+		int rc = wrapper_bytes(ctx, held, have, s->format, &hb);
+		if (rc) return rc;
 		if (hb == -1) r = LDB_BAD_DATA;
 		else if (hb >= 0) { header = true; used = (size_t)hb; }
 	}
