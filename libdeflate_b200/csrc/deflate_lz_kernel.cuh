@@ -16,7 +16,8 @@
 // lives in shared memory (~224 KiB):
 //   * a 64 KiB ring of the input (the sliding window), filled 16 KiB at a time by the
 //     TMA bulk-copy engine (cp.async.bulk + mbarrier) -- the window never touches
-//     HBM again,
+//     HBM again; its first 512 bytes are mirrored past its end (LZ_RING_GUARD), so the search reads a
+//     match at pos & 0xffff onwards without masking every access,
 //   * 13-bit hash heads (u16[8192]) and a chain table with one slot per position
 //     mod 65536 (u16[65536]); a pass is 16 Ki positions and the window 32 Ki, so the
 //     16 Ki slots of the FOLLOWING pass are always dead and serve as scratch,
@@ -52,6 +53,7 @@
 #define LZ_NSL       (1 << LZ_NSL_BITS)
 #define LZ_SEG       16384			// largest single TMA load
 #define LZ_RING      65536
+#define LZ_RING_GUARD 512			// ring[0, GUARD) mirrored at ring[RING, RING + GUARD) (lz_load_segment)
 #define LZ_HASH_BITS 13
 #define LZ_WIN       32768
 #define LZ_LOOKAHEAD 512			// bytes past the pass kept in the ring (>= 258 + 8)
@@ -118,7 +120,7 @@ static_assert(LZ_GROUP_FLUSH >= LZ_GROUP_MIN_FLUSH && LZ_GROUP_FLUSH <= LZ_GROUP
 
 // shared memory layout
 #define LZ_SM_RING   0
-#define LZ_SM_NEXT   (LZ_SM_RING + LZ_RING)			// u16[65536], indexed by pos mod 65536
+#define LZ_SM_NEXT   (LZ_SM_RING + LZ_RING + LZ_RING_GUARD)	// u16[65536], indexed by pos mod 65536
 #define LZ_SM_HEAD   (LZ_SM_NEXT + 2 * 65536)			// u16[1 << HASH_BITS]
 #define LZ_SM_R      (LZ_SM_HEAD + 2 * (1 << LZ_HASH_BITS))	// 12 KiB multi-purpose region:
 #define LZ_SM_VIS    (LZ_SM_R)					//   parse: u32[NWIN] visited masks
@@ -132,6 +134,9 @@ static_assert(LZ_GROUP_FLUSH >= LZ_GROUP_MIN_FLUSH && LZ_GROUP_FLUSH <= LZ_GROUP
 #define LZ_SM_CODES  (LZ_SM_LENS + 320)				// u16[320]
 #define LZ_SM_VARS   (LZ_SM_CODES + 2 * 320)			// misc scalars, mbarrier
 #define LZ_SM_BYTES  (LZ_SM_VARS + 256)
+static_assert(LZ_SM_BYTES <= 232448, "the layout fits the opt-in shared memory of one sm_90 CTA");
+static_assert(LZ_RING_GUARD % 16 == 0 && LZ_RING_GUARD >= 258 + 16, "the guard keeps the layout 16-byte aligned and "
+	      "covers a 258-byte match read 8 bytes at a time (lz_match_len)");
 
 // per-CTA global scratch (L2 resident): per-position results of the current pass + tokens
 #define LZ_BLOCK_POS (LZ_BLOCK_PASSES * LZ_PASS)		// positions per block
@@ -232,6 +237,39 @@ __device__ __forceinline__ u32 lz_ld32(const u8 *ring, u32 pos)
 	return __funnelshift_r(lo, hi, (a & 3) * 8);
 }
 __device__ __forceinline__ u32 lz_ld8(const u8 *ring, u32 pos) { return ring[pos & (LZ_RING - 1)]; }
+// The 4 bytes at ring index a, unmasked: a + 8 <= LZ_RING + LZ_RING_GUARD (a = pos & (LZ_RING - 1) plus a short reach)
+__device__ __forceinline__ u32 lz_ld32u(const u8 *ring, u32 a)
+{
+	const u32 *w = (const u32 *)ring + (a >> 2);
+	return __funnelshift_r(w[0], w[1], (a & 3) * 8);
+}
+// The first k in [len, max_len) with ring[a + k] != ring[b + k], else max_len (len itself when it is not below
+// max_len), 8 bytes per trip.  a and b are ring indexes (< LZ_RING) and max_len <= 258, so every word read, up
+// to a + max_len + 11, lies in the ring or its guard; bytes at and past max_len may be stale and only ever
+// decide a length that is then capped.
+__device__ __forceinline__ u32 lz_match_len(const u8 *ring, u32 a, u32 b, u32 len, u32 max_len)
+{
+	if (len >= max_len) return len;
+	const u32 *wa = (const u32 *)ring + ((a + len) >> 2), *wb = (const u32 *)ring + ((b + len) >> 2);
+	const u32 sa = ((a + len) & 3) * 8, sb = ((b + len) & 3) * 8;
+	u32 a0 = wa[0], b0 = wb[0];
+	for (;;) {
+		const u32 a1 = wa[1], a2 = wa[2], b1 = wb[1], b2 = wb[2];
+		const u32 x0 = __funnelshift_r(a0, a1, sa) ^ __funnelshift_r(b0, b1, sb);
+		const u32 x1 = __funnelshift_r(a1, a2, sa) ^ __funnelshift_r(b1, b2, sb);
+		if (x0 | x1) {
+			len += x0 ? (__ffs(x0) - 1) >> 3 : 4 + ((__ffs(x1) - 1) >> 3);
+			break;
+		}
+		len += 8;
+		if (len >= max_len) break;
+		wa += 2;
+		wb += 2;
+		a0 = a2;
+		b0 = b2;
+	}
+	return len < max_len ? len : max_len;
+}
 __device__ __forceinline__ u32 lz_hash(u32 v) { return (v * 0x1E35A7BDu) >> (32 - LZ_HASH_BITS); }	// ref: matchfinder_common.h:168-172
 
 // ---- length / offset slot helpers (Appendix A; ref: deflate_compress.c:237-308) ------
@@ -288,6 +326,10 @@ __device__ __forceinline__ void lz_load_segment(const lz_group &g, u8 *sm, const
 	for (u32 i = bulk + g.tid; i < len; i += g.gt) ring[(from + i) & (LZ_RING - 1)] = in[from + i];
 	g.sync();
 	if (bulk && g.tid == 0) v->tma_phase ^= 1;
+	// the guard: the bytes of ring[0, LZ_RING_GUARD) this load wrote, again past the ring's end, so that a
+	// reader may index ring + (pos & (LZ_RING - 1)) + k for k < LZ_RING_GUARD without wrapping
+	const u32 lo = from & (LZ_RING - 1), hi = lo + len < LZ_RING_GUARD ? lo + len : LZ_RING_GUARD;
+	for (u32 i = lo + g.tid; i < hi; i += g.gt) ring[LZ_RING + i] = ring[i];
 	g.sync();
 }
 

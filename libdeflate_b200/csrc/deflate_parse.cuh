@@ -18,16 +18,17 @@ __device__ __forceinline__ void lz_search(const u8 *ring, const u16 *nextt, u32 
 {
 	const u32 max_len = n - p < 258 ? n - p : 258;
 	const u32 nice = nice_level < max_len ? nice_level : max_len;
-	if (best_len) {
-		// a carried-over match may continue past where its predecessor was capped
-		while (best_len < max_len && lz_ld8(ring, p + best_len) == lz_ld8(ring, p - best_dist + best_len)) best_len++;
-	}
+	const u32 pa = p & (LZ_RING - 1);	// p's ring index: every read below reaches into the guard, not around the ring
+	// a carried-over match may continue past where its predecessor was capped
+	if (best_len) best_len = lz_match_len(ring, pa, (p - best_dist) & (LZ_RING - 1), best_len, max_len);
 	if (best_len >= nice) return;
-	const u32 cur = lz_ld32(ring, p);
+	// p's bytes [0, 4) and [4, 12), the latter kept for the extension of every candidate
+	const u32 *pw = (const u32 *)ring + (pa >> 2), ps = (pa & 3) * 8, w1 = pw[1], w2 = pw[2];
+	const u32 cur = __funnelshift_r(pw[0], w1, ps), pe0 = __funnelshift_r(w1, w2, ps), pe1 = __funnelshift_r(w2, pw[3], ps);
 	u32 tailo = best_len >= 4 ? best_len - 3 : 0;
-	u32 tailv = tailo ? lz_ld32(ring, p + tailo) : cur;
+	u32 tailv = tailo ? lz_ld32u(ring, pa + tailo) : cur;
 	const u32 lim = p < LZ_MAX_DIST ? p : LZ_MAX_DIST;
-	u32 cand = nextt[p & 0xffff];
+	u32 cand = nextt[pa];
 	u32 prev_dist = 0;
 	for (int d = 0; d < depth; d++) {
 		const u32 dist = (p - cand) & 0xffff;
@@ -35,23 +36,23 @@ __device__ __forceinline__ void lz_search(const u8 *ring, const u16 *nextt, u32 
 		prev_dist = dist;
 		const u32 cq = cand;			// ring index of the candidate (positions are stored mod 65536)
 		cand = nextt[cq];
-		if (lz_ld8(ring, cq + tailo + 3) != (tailv >> 24)) continue;
-		if (lz_ld32(ring, cq + tailo) != tailv) continue;
-		if (tailo && lz_ld32(ring, cq) != cur) continue;
-		u32 len = 4;
-		while (len + 4 <= max_len) {
-			u32 x = lz_ld32(ring, p + len) ^ lz_ld32(ring, cq + len);
-			if (x) { len += (__ffs(x) - 1) >> 3; goto extended; }
-			len += 4;
+		if (ring[cq + tailo + 3] != (tailv >> 24)) continue;
+		if (lz_ld32u(ring, cq + tailo) != tailv) continue;
+		if (tailo && lz_ld32u(ring, cq) != cur) continue;
+		u32 len;
+		{
+			const u32 x0 = pe0 ^ lz_ld32u(ring, cq + 4), x1 = pe1 ^ lz_ld32u(ring, cq + 8);
+			if (x0) len = 4 + ((__ffs(x0) - 1) >> 3);
+			else if (x1) len = 8 + ((__ffs(x1) - 1) >> 3);
+			else len = lz_match_len(ring, pa, cq, 12, max_len);
+			if (len > max_len) len = max_len;
 		}
-		while (len < max_len && lz_ld8(ring, p + len) == lz_ld8(ring, cq + len)) len++;
-	extended:
 		if (len > best_len) {
 			best_len = len;
 			best_dist = dist;
 			if (len >= nice) break;
 			tailo = len - 3;
-			tailv = lz_ld32(ring, p + tailo);
+			tailv = lz_ld32u(ring, pa + tailo);
 		}
 	}
 }
@@ -66,12 +67,14 @@ __device__ __forceinline__ void lz_search_all(const u8 *ring, const u16 *nextt, 
 {
 	const u32 max_len = n - p < 258 ? n - p : 258;
 	const u32 nice = nice_level < max_len ? nice_level : max_len;
-	const u32 cur = lz_ld32(ring, p);
+	const u32 pa = p & (LZ_RING - 1);
+	const u32 *pw = (const u32 *)ring + (pa >> 2), ps = (pa & 3) * 8, w1 = pw[1], w2 = pw[2];
+	const u32 cur = __funnelshift_r(pw[0], w1, ps), pe0 = __funnelshift_r(w1, w2, ps), pe1 = __funnelshift_r(w2, pw[3], ps);
 	u32 tailo = 0, tailv = cur, cnt = 0;
 	best_len = 0;
 	best_dist = 0;
 	const u32 lim = p < LZ_MAX_DIST ? p : LZ_MAX_DIST;
-	u32 cand = nextt[p & 0xffff];
+	u32 cand = nextt[pa];
 	u32 prev_dist = 0;
 	for (int d = 0; d < depth; d++) {
 		const u32 dist = (p - cand) & 0xffff;
@@ -79,17 +82,17 @@ __device__ __forceinline__ void lz_search_all(const u8 *ring, const u16 *nextt, 
 		prev_dist = dist;
 		const u32 cq = cand;
 		cand = nextt[cq];
-		if (lz_ld8(ring, cq + tailo + 3) != (tailv >> 24)) continue;
-		if (lz_ld32(ring, cq + tailo) != tailv) continue;
-		if (tailo && lz_ld32(ring, cq) != cur) continue;
-		u32 len = 4;
-		while (len + 4 <= max_len) {
-			u32 x = lz_ld32(ring, p + len) ^ lz_ld32(ring, cq + len);
-			if (x) { len += (__ffs(x) - 1) >> 3; goto extended; }
-			len += 4;
+		if (ring[cq + tailo + 3] != (tailv >> 24)) continue;
+		if (lz_ld32u(ring, cq + tailo) != tailv) continue;
+		if (tailo && lz_ld32u(ring, cq) != cur) continue;
+		u32 len;
+		{
+			const u32 x0 = pe0 ^ lz_ld32u(ring, cq + 4), x1 = pe1 ^ lz_ld32u(ring, cq + 8);
+			if (x0) len = 4 + ((__ffs(x0) - 1) >> 3);
+			else if (x1) len = 8 + ((__ffs(x1) - 1) >> 3);
+			else len = lz_match_len(ring, pa, cq, 12, max_len);
+			if (len > max_len) len = max_len;
 		}
-		while (len < max_len && lz_ld8(ring, p + len) == lz_ld8(ring, cq + len)) len++;
-	extended:
 		if (len > best_len) {
 			best_len = len;
 			best_dist = dist;
@@ -97,7 +100,7 @@ __device__ __forceinline__ void lz_search_all(const u8 *ring, const u16 *nextt, 
 			cnt++;
 			if (len >= nice) break;
 			tailo = len - 3;
-			tailv = lz_ld32(ring, p + tailo);
+			tailv = lz_ld32u(ring, pa + tailo);
 		}
 	}
 	for (u32 k = cnt; k < LZ_OPT_K; k++) ml[k] = 0;
@@ -266,8 +269,10 @@ __device__ __forceinline__ void lz_search_pass(u8 *sm, const lz_params &P, int l
 			for (u32 k = i + 1; k < stop; k++) {
 				const u32 pk = b0 + k;
 				// (the match ended on a mismatch unless it was capped at 258 bytes)
-				if (mL == 258)
-					while (mend < nn && mend - pk < 258 && lz_ld8(ring, mend) == lz_ld8(ring, mend - mD)) mend++;
+				if (mL == 258 && mend < nn && mend - pk < 258) {
+					const u32 cap = nn - pk < 258 ? nn - pk : 258;
+					mend = pk + lz_match_len(ring, pk & (LZ_RING - 1), (pk - mD) & (LZ_RING - 1), mend - pk, cap);
+				}
 				u32 lk = mend - pk;
 				rs[k] = lk >= 4 ? lk | ((mD - 1) << 16) : 0;
 			}
