@@ -411,7 +411,7 @@ libdeflate_b200_decompress_stream_write_host(struct libdeflate_b200_decompress_s
  *   Point 0 is the first DEFLATE bit after the wrapper, at output 0; after it, the first chain start whose
  *   output offset is at least 'spacing' past the previous point and at least 32 KiB.  A point records its
  *   input bit, its output offset, the CRC-32 of its span (the output up to the next point) and the 32 KiB of
- *   output before it (device memory).  A stream that decompress_large decodes as one segment gets one point,
+ *   output before it (device memory; host memory for an index from a decompress stream or index_load_ex).  A stream that decompress_large decodes as one segment gets one point,
  *   and every extract from it is a one-lane decode of the whole stream.  gzip: the first member only.
  *
  * index_build: decodes exactly as decompress_large does (same bytes in d_out; *result, *actual_in and
@@ -435,7 +435,27 @@ libdeflate_b200_decompress_stream_write_host(struct libdeflate_b200_decompress_s
  *   the first needed point to the end of the last needed span, plus LIBDEFLATE_B200_INDEX_READ_MARGIN bytes.
  *   It returns an error code, having done nothing, when a range passes index_out_nbytes or in_nbytes is not
  *   the indexed stream's.  It WAITS, as decompress_large does.
- * index_extract_host: host input and destinations; only the input bytes the decode reads are staged.
+ * index_extract_host: host input and destinations.  Each decode wave stages only the input of its own spans:
+ *   every run of consecutive needed spans, from its point's byte to its end plus
+ *   LIBDEFLATE_B200_INDEX_READ_MARGIN, packed.  The input staged at once is at most 1 GiB, or one span when a
+ *   span is larger, however far apart the ranges lie in the stream.
+ *
+ * An index of a stream larger than the card, built as a decompress stream reads it:
+ * decompress_stream_create_indexed: a decompress stream that is byte for byte the plain one (same output,
+ *   results, pending() and trailer check) and collects an index as it goes, with the access point rule above
+ *   applied to the chain segments of every write (a write's first segment included; only output a write
+ *   delivers counts).  spacing as for index_build.  The windows of the points go to host memory at every
+ *   write, through the context's pinned memory: the stream holds no device memory beyond a plain stream's,
+ *   and the index costs 32 KiB of host memory per point (1/8 of the output at the default spacing).
+ * decompress_stream_take_index: after a write returned LIBDEFLATE_SUCCESS, a new index of the stream (the
+ *   caller destroys it with index_destroy); its in_nbytes and actual_in are the stream's bytes through its
+ *   trailer (the bytes after it are not part of it).  NULL, with last_error() saying why, before that, after
+ *   BAD_DATA, on a plain stream or when taken already.  Its windows are in host memory; every index call
+ *   works on it, and its blob is the same as index_build's would be.  Points where writes split the stream
+ *   are block starts, not always sync points: such an index stops its spans at any block header on a point.
+ * index_load_ex: index_load, with the windows kept in host memory when flags has
+ *   LIBDEFLATE_B200_INDEX_HOST_WINDOWS (for indexes whose windows do not fit on the card); flags 0 is
+ *   index_load.  An extract from an index with host windows copies each wave's windows to the device.
  * Kernel time: decode as kind 2, resolve as kind 5, span CRCs as kind 0, the copies (windows, prefixes,
  * ranges) as kind 6; index_build adds the kinds of decompress_large.
  */
@@ -462,6 +482,9 @@ LIBDEFLATEAPI int
 libdeflate_b200_index_serialize(const struct libdeflate_b200_index *ix, void *buf, size_t avail);
 LIBDEFLATEAPI struct libdeflate_b200_index *
 libdeflate_b200_index_load(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes);
+#define LIBDEFLATE_B200_INDEX_HOST_WINDOWS 1u
+LIBDEFLATEAPI struct libdeflate_b200_index *
+libdeflate_b200_index_load_ex(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes, unsigned flags);
 LIBDEFLATEAPI int
 libdeflate_b200_index_extract(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *d_in,
 			      size_t in_nbytes, const uint64_t *h_offsets, const size_t *h_lens, void *const *d_dst,
@@ -470,6 +493,10 @@ LIBDEFLATEAPI int
 libdeflate_b200_index_extract_host(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *in,
 				   size_t in_nbytes, const uint64_t *h_offsets, const size_t *h_lens, void *const *h_dst,
 				   int32_t *h_results, size_t n_ranges);
+LIBDEFLATEAPI struct libdeflate_b200_decompress_stream *
+libdeflate_b200_decompress_stream_create_indexed(struct libdeflate_b200_ctx *ctx, int format, size_t spacing);
+LIBDEFLATEAPI struct libdeflate_b200_index *
+libdeflate_b200_decompress_stream_take_index(struct libdeflate_b200_decompress_stream *s);
 
 #ifdef __cplusplus
 }

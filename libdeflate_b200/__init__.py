@@ -59,11 +59,13 @@ BATCH_SYMBOLS = [
     "libdeflate_b200_index_build", "libdeflate_b200_index_build_host", "libdeflate_b200_index_destroy",
     "libdeflate_b200_index_points", "libdeflate_b200_index_out_nbytes", "libdeflate_b200_index_serialized_size",
     "libdeflate_b200_index_serialize", "libdeflate_b200_index_load", "libdeflate_b200_index_extract",
-    "libdeflate_b200_index_extract_host",
+    "libdeflate_b200_index_extract_host", "libdeflate_b200_index_load_ex",
+    "libdeflate_b200_decompress_stream_create_indexed", "libdeflate_b200_decompress_stream_take_index",
 ]
 LARGE_PIECE = 131072    # LIBDEFLATE_B200_LARGE_PIECE: input bytes per piece of compress_large
 INDEX_SPACING = 262144      # LIBDEFLATE_B200_INDEX_SPACING: default output bytes between access points
 INDEX_READ_MARGIN = 16      # LIBDEFLATE_B200_INDEX_READ_MARGIN: input an extract may read past its last span
+INDEX_HOST_WINDOWS = 1      # LIBDEFLATE_B200_INDEX_HOST_WINDOWS: index_load_ex keeps the windows in host memory
 NO_FLUSH, SYNC_FLUSH, FINISH = 0, 1, 2     # flush modes of a compress stream's write
 SUCCESS, BAD_DATA = 0, 1                   # libdeflate results
 MORE_INPUT, MORE_OUTPUT = 0x100, 0x101     # the other results of a decompress stream's write
@@ -199,6 +201,10 @@ def load_library(path=None):
     lib.libdeflate_b200_compress_stream_write_host.argtypes = [P, P, S, c_int, P, S, PS]
     lib.libdeflate_b200_decompress_stream_create.restype = P
     lib.libdeflate_b200_decompress_stream_create.argtypes = [P, c_int]
+    lib.libdeflate_b200_decompress_stream_create_indexed.restype = P
+    lib.libdeflate_b200_decompress_stream_create_indexed.argtypes = [P, c_int, S]
+    lib.libdeflate_b200_decompress_stream_take_index.restype = P
+    lib.libdeflate_b200_decompress_stream_take_index.argtypes = [P]
     lib.libdeflate_b200_decompress_stream_destroy.restype = None
     lib.libdeflate_b200_decompress_stream_destroy.argtypes = [P]
     lib.libdeflate_b200_decompress_stream_pending.restype = S
@@ -223,6 +229,8 @@ def load_library(path=None):
     lib.libdeflate_b200_index_serialize.argtypes = [P, P, S]
     lib.libdeflate_b200_index_load.restype = P
     lib.libdeflate_b200_index_load.argtypes = [P, P, S]
+    lib.libdeflate_b200_index_load_ex.restype = P
+    lib.libdeflate_b200_index_load_ex.argtypes = [P, P, S, c_uint]
     for f in ("extract", "extract_host"):
         fn = getattr(lib, "libdeflate_b200_index_" + f)
         fn.restype = c_int
@@ -253,6 +261,14 @@ def _buf_ptr(b):
     mv = memoryview(b).cast("B")
     arr = (ctypes.c_char * len(mv)).from_buffer(mv) if not mv.readonly else (ctypes.c_char * len(mv)).from_buffer_copy(mv)
     return ctypes.addressof(arr), len(mv), arr
+
+
+def _ro_buf_ptr(b):
+    """(address, length, keepalive) of a contiguous bytes-like object that is only read, never copied: bytes,
+    read-only buffers and mmaps of files larger than host memory included."""
+    import numpy as np
+    a = np.frombuffer(memoryview(b).cast("B"), np.uint8)
+    return a.ctypes.data, a.size, a
 
 
 class Api:
@@ -488,10 +504,12 @@ class Context:
             return res.value, None, 0, 0, None
         return SUCCESS, ctypes.string_at(out, aout.value), ain.value, aout.value, Index(self, ix.value)
 
-    def load_index(self, blob):
-        """The Index of a serialized blob (Index.to_bytes()); raises Error when the blob is malformed."""
+    def load_index(self, blob, host_windows=False):
+        """The Index of a serialized blob (Index.to_bytes()); raises Error when the blob is malformed.
+        host_windows: keep its windows in host memory (index_load_ex), for indexes whose windows do not fit
+        on the card."""
         addr, n, keep = _buf_ptr(blob)
-        h = self.l.libdeflate_b200_index_load(self.h, addr, n)
+        h = self.l.libdeflate_b200_index_load_ex(self.h, addr, n, INDEX_HOST_WINDOWS if host_windows else 0)
         if not h:
             raise Error("index_load failed: %s" % self.l.libdeflate_b200_last_error().decode())
         return Index(self, h)
@@ -500,9 +518,10 @@ class Context:
         """A CompressStream on this context: ONE stream written call by call, like zlib.compressobj."""
         return CompressStream(self, level, fmt)
 
-    def decompressobj(self, fmt=RAW):
-        """A DecompressStream on this context: ONE stream read call by call, like zlib.decompressobj."""
-        return DecompressStream(self, fmt)
+    def decompressobj(self, fmt=RAW, index_spacing=None):
+        """A DecompressStream on this context: ONE stream read call by call, like zlib.decompressobj.
+        index_spacing: an int makes it collect an Index as it goes (DecompressStream.index(); 0: INDEX_SPACING)."""
+        return DecompressStream(self, fmt, index_spacing)
 
     def large_segments(self):
         """Segments the last decompress_large decoded in parallel (1: one lane)."""
@@ -608,8 +627,9 @@ class Index:
         return buf.raw
 
     def read(self, data, ranges):
-        """[(result, bytes or None)] for each (offset, length) of 'ranges', from the indexed stream 'data' (host)."""
-        addr, n, keep = _buf_ptr(data)
+        """[(result, bytes or None)] for each (offset, length) of 'ranges', from the indexed stream 'data' (host;
+        any contiguous buffer, e.g. a read-only mmap of the file, which is not copied)."""
+        addr, n, keep = _ro_buf_ptr(data)
         k = len(ranges)
         offs = (c_uint64 * max(k, 1))(*[o for o, _ in ranges])
         lens = (c_size_t * max(k, 1))(*[ln for _, ln in ranges])
@@ -695,10 +715,13 @@ class DecompressStream:
     bytes, flush() -> bytes (a write of nothing with 'last' set), eof, unused_data, pending.  Every call decodes
     the complete blocks it can with the whole GPU.  Host buffers."""
 
-    def __init__(self, ctx, fmt=RAW):
+    def __init__(self, ctx, fmt=RAW, index_spacing=None):
         self.ctx = ctx
         self.l = ctx.l
-        self.h = self.l.libdeflate_b200_decompress_stream_create(ctx.h, fmt)
+        if index_spacing is None:
+            self.h = self.l.libdeflate_b200_decompress_stream_create(ctx.h, fmt)
+        else:
+            self.h = self.l.libdeflate_b200_decompress_stream_create_indexed(ctx.h, fmt, index_spacing)
         if not self.h:
             raise Error("decompress_stream_create(fmt=%d) failed: %s" % (fmt, self.l.libdeflate_b200_last_error().decode()))
         ctx._streams.add(self)
@@ -781,6 +804,14 @@ class DecompressStream:
         if self.eof:
             return self._drain_buf(0)
         return self._drain(b"", True, 0)
+
+    def index(self):
+        """The Index an indexed stream (Context.decompressobj(fmt, index_spacing)) collected, once it has ended
+        (eof): once per stream.  Raises Error otherwise."""
+        h = self.l.libdeflate_b200_decompress_stream_take_index(self.h) if self.h else None
+        if not h:
+            raise Error("decompress_stream_take_index failed: %s" % self.l.libdeflate_b200_last_error().decode())
+        return Index(self.ctx, h)
 
     def close(self):
         if self.h:

@@ -70,7 +70,7 @@ def build(verbose=False, force=False):
 
 def build_emu(force=False):
     """g++ build of the same sources against the SIMT emulator (tests only)."""
-    deps = _deps() + [os.path.join(EMU_DIR, "cuda_emu.h"), os.path.join(EMU_DIR, "cuda_emu.cpp")]
+    deps = _deps() + [os.path.join(EMU_DIR, f) for f in ("cuda_emu.h", "cuda_emu.cpp", "alloc_probe.cpp")]
     if not force and not _newer(EMU_LIB, deps):
         return EMU_LIB
     os.makedirs(os.path.dirname(EMU_LIB), exist_ok=True)
@@ -82,9 +82,10 @@ def build_emu(force=False):
         obj = os.path.join(os.path.dirname(EMU_LIB), src.replace(".cu", ".emu.o"))
         procs.append(subprocess.Popen(common + ["-x", "c++", "-c", os.path.join(CSRC, src), "-o", obj]))
         objs.append(obj)
-    obj = os.path.join(os.path.dirname(EMU_LIB), "cuda_emu.o")
-    procs.append(subprocess.Popen(common + ["-c", os.path.join(EMU_DIR, "cuda_emu.cpp"), "-o", obj]))
-    objs.append(obj)
+    for src in ("cuda_emu.cpp", "alloc_probe.cpp"):
+        obj = os.path.join(os.path.dirname(EMU_LIB), src.replace(".cpp", ".o"))
+        procs.append(subprocess.Popen(common + ["-c", os.path.join(EMU_DIR, src), "-o", obj]))
+        objs.append(obj)
     for p in procs:
         if p.wait() != 0:
             raise RuntimeError("emu build failed")

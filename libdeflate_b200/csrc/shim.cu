@@ -114,6 +114,7 @@ struct libdeflate_b200_ctx {
 	ldb_buf d_params;		// device: pointer/size arrays for host-buffer calls
 	ldb_buf h_pinned;		// pinned host staging
 	ldb_buf h_pinned_tab;		// pinned host: size / offset tables read back while kernels keep running
+	ldb_buf h_win;			// pinned host: index windows on their way to or from host memory
 	u64 launches;
 	cudaEvent_t ev_start, ev_stop;
 	cudaStream_t stream_h2d, stream_d2h;	// copy streams of the pipelined host-buffer path
@@ -241,6 +242,7 @@ extern "C" void libdeflate_b200_ctx_destroy(struct libdeflate_b200_ctx *ctx)
 	cudaFree(ctx->d_params.p);
 	if (ctx->h_pinned.p) cudaFreeHost(ctx->h_pinned.p);
 	if (ctx->h_pinned_tab.p) cudaFreeHost(ctx->h_pinned_tab.p);
+	if (ctx->h_win.p) cudaFreeHost(ctx->h_win.p);
 	delete ctx;
 }
 
@@ -1611,16 +1613,24 @@ struct li_run {
 	u64 out;		// output bytes written
 };
 
-// ---- the index's access points, collected wave by wave (DESIGN.md 4.9) ----------------------------------
+// ---- the index's access points, collected wave by wave (DESIGN.md 4.9, 4.10) ----------------------------
 // Point 0 is the first DEFLATE bit at output 0 (the caller fills its bit).  A chain segment's start becomes the
 // next point when its G is at least 'spacing' past the previous point and at least 32 KiB: its window is then
-// the full W_k, which the wave's window chain has just written and the next wave overwrites.
+// the full W_k, which the wave's window chain has just written and the next wave overwrites.  A decompress
+// stream feeds one sink from every write: out0 / bit0 place the write's chain in the stream, and the windows
+// go to host memory.
 struct li_index_sink {
 	u64 spacing;
 	std::vector<u64> bit, out;	// the points
 	bool any_header = false;	// they are found block starts (ldb_seg_args.any_header)
+	bool block_start = false;	// a point after point 0 is not a sync point from the split scan
+	u64 out0 = 0, bit0 = 0;		// the stream's output byte and input bit where the call's chain starts
 	u8 *d_win = nullptr;		// the windows of points 1, 2, ... (32 KiB each); owned by the sink until taken
 	size_t win_cap = 0;		// windows d_win holds room for
+	bool host = false;		// the windows go to h_win instead, through the context's pinned h_win
+	std::vector<u8> h_win;
+	std::vector<u32> crc;		// decompress stream: the CRC-32s of the closed spans ...
+	u32 span_crc = 0;		// ... and of the open one so far
 	~li_index_sink() { cudaFree(d_win); }
 };
 
@@ -1636,17 +1646,35 @@ static int li_copy(libdeflate_b200_ctx *ctx, const std::vector<ldb_copy_piece> &
 	return ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_copy_pieces(d, pc.size(), ctx->stream); });
 }
 
-// One wave's chain segments recs[0, nc), whose windows W before each are at win + m x 32 KiB
-static int li_index_take(libdeflate_b200_ctx *ctx, li_index_sink &ix, const li_chain_rec *recs, size_t nc, const u8 *win)
+// One wave's chain segments recs[0, nc), whose windows W before each are at win + m x 32 KiB.  first: the
+// call's chain records before recs[0]; sync: the call's split points are sync points.  (A call's first chain
+// segment starts at a block it was given, which need not be a sync point.)
+static int li_index_take(libdeflate_b200_ctx *ctx, li_index_sink &ix, const li_chain_rec *recs, size_t nc, const u8 *win,
+			 size_t first, bool sync)
 {
 	std::vector<size_t> take;
-	for (size_t m = 0; m < nc; m++)
-		if (recs[m].G >= LDB_SEG_PREFIX && recs[m].G - ix.out.back() >= ix.spacing) {
-			ix.bit.push_back(recs[m].start);
-			ix.out.push_back(recs[m].G);
+	for (size_t m = 0; m < nc; m++) {
+		const u64 G = ix.out0 + recs[m].G;
+		if (G >= LDB_SEG_PREFIX && G - ix.out.back() >= ix.spacing) {
+			ix.bit.push_back(ix.bit0 + recs[m].start);
+			ix.out.push_back(G);
 			take.push_back(m);
+			if (!sync || first + m == 0) ix.block_start = true;
 		}
+	}
 	if (take.empty()) return 0;
+	if (ix.host) {	// gathered into pinned memory by the copy kernel, then appended
+		int rc = ldb_reserve_pinned(ctx->h_win, take.size() * (size_t)LDB_SEG_PREFIX);
+		if (rc) return rc;
+		std::vector<ldb_copy_piece> pc;
+		for (size_t i = 0; i < take.size(); i++)
+			pc.push_back({win + take[i] * (size_t)LDB_SEG_PREFIX, (u8 *)ctx->h_win.p + i * (size_t)LDB_SEG_PREFIX, LDB_SEG_PREFIX});
+		rc = li_copy(ctx, pc);
+		if (rc) return rc;
+		LDB_CUDA_CHECK_RET(cudaStreamSynchronize(ctx->stream));
+		ix.h_win.insert(ix.h_win.end(), (const u8 *)ctx->h_win.p, (const u8 *)ctx->h_win.p + take.size() * (size_t)LDB_SEG_PREFIX);
+		return 0;
+	}
 	const size_t nw = ix.out.size() - 1;
 	if (nw > ix.win_cap) {		// grown by doubling, the windows so far kept
 		const size_t cap = std::max(nw, 2 * ix.win_cap);
@@ -1931,7 +1959,7 @@ static int li_chain(libdeflate_b200_ctx *ctx, const li_call &call, li_run *run)
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(win, ctx->li_carry.p, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
 		rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_window_chain((const ldb_chain_seg *)d_cs, nc, win, ctx->stream); });
 		if (!rc) rc = ldb_timed_launch(ctx, LDB_K_PACK, [&] { return ldb_launch_substitute((const ldb_chain_seg *)d_cs, nc, win, ctx->stream); });
-		if (!rc && call.index) rc = li_index_take(ctx, *call.index, chain.data() + chain.size() - nc, nc, win);
+		if (!rc && call.index) rc = li_index_take(ctx, *call.index, chain.data() + chain.size() - nc, nc, win, chain.size() - nc, !found);
 		if (rc) return rc;
 		LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_carry.p, win + nc * (size_t)LDB_SEG_PREFIX, LDB_SEG_PREFIX, cudaMemcpyDeviceToDevice, ctx->stream));
 		// (the next wave reuses these buffers)
@@ -2065,7 +2093,9 @@ struct libdeflate_b200_index {
 	u64 in_nbytes, actual_in, out_nbytes, spacing;
 	std::vector<u64> bit, out;	// per point: its first input bit, its output offset
 	std::vector<u32> crc;		// per point: the CRC-32 of its span, [out[p], out[p + 1] or out_nbytes)
-	u8 *d_win;			// windows of points 1, 2, ...: 32 KiB each (device)
+	u8 *d_win;			// windows of points 1, 2, ...: 32 KiB each, on the device ...
+	bool host_win;			// ... or in host memory (h_win)
+	std::vector<u8> h_win;
 };
 
 static u32 h_crc32(const u8 *p, size_t n)
@@ -2094,6 +2124,7 @@ static libdeflate_b200_index *index_new(libdeflate_b200_ctx *ctx)
 	libdeflate_b200_index *ix = new libdeflate_b200_index();
 	ix->ctx = ctx;
 	ix->d_win = nullptr;
+	ix->host_win = false;
 	return ix;
 }
 
@@ -2222,16 +2253,22 @@ extern "C" int libdeflate_b200_index_serialize(const struct libdeflate_b200_inde
 		put32(t + 16, ix->crc[p]);
 		put32(t + 20, 0);
 	}
-	int rc = read_back(ix->ctx, t, ix->d_win, (np - 1) * (size_t)LDB_SEG_PREFIX);
-	if (rc) return rc;
+	if (ix->host_win) {
+		if (np > 1) memcpy(t, ix->h_win.data(), (np - 1) * (size_t)LDB_SEG_PREFIX);
+	} else {
+		int rc = read_back(ix->ctx, t, ix->d_win, (np - 1) * (size_t)LDB_SEG_PREFIX);
+		if (rc) return rc;
+	}
 	put32(b + total - 4, h_crc32(b, total - 4));
 	return 0;
 }
 
-extern "C" struct libdeflate_b200_index *libdeflate_b200_index_load(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes)
+extern "C" struct libdeflate_b200_index *libdeflate_b200_index_load_ex(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes,
+									unsigned flags)
 {
 	auto bad = [](const char *why) -> libdeflate_b200_index * { ldb_fail(cudaErrorInvalidValue, why, __FILE__, __LINE__); return nullptr; };
 	if (!ctx || (!buf && nbytes)) return bad("index_load: no context or buffer");
+	if (flags & ~LIBDEFLATE_B200_INDEX_HOST_WINDOWS) return bad("index_load_ex: unknown flags");
 	const u8 *b = (const u8 *)buf;
 	if (nbytes < LI_INDEX_HEADER + LI_INDEX_POINT + 4) return bad("index_load: shorter than an index");
 	if (get32(b) != LI_INDEX_MAGIC) return bad("index_load: not an index (magic)");
@@ -2263,6 +2300,11 @@ extern "C" struct libdeflate_b200_index *libdeflate_b200_index_load(struct libde
 		ix->crc.push_back(get32(t + 16));
 	}
 	const size_t wb = (size_t)(np - 1) * LDB_SEG_PREFIX;
+	if (flags & LIBDEFLATE_B200_INDEX_HOST_WINDOWS) {
+		ix->host_win = true;
+		ix->h_win.assign(t, t + wb);
+		return ix;
+	}
 	cudaError_t e = cudaSetDevice(ctx->device);
 	if (e == cudaSuccess && wb) e = cudaMalloc((void **)&ix->d_win, wb);
 	if (e == cudaSuccess && wb) e = cudaMemcpy(ix->d_win, t, wb, cudaMemcpyHostToDevice);
@@ -2272,6 +2314,11 @@ extern "C" struct libdeflate_b200_index *libdeflate_b200_index_load(struct libde
 		return nullptr;
 	}
 	return ix;
+}
+
+extern "C" struct libdeflate_b200_index *libdeflate_b200_index_load(struct libdeflate_b200_ctx *ctx, const void *buf, size_t nbytes)
+{
+	return libdeflate_b200_index_load_ex(ctx, buf, nbytes, 0);
 }
 
 // ---- extract ------------------------------------------------------------------------------------------
@@ -2310,35 +2357,30 @@ static int li_plan_of(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix,
 	return 0;
 }
 
-// 'in' holds the stream's bytes [pl.lo, pl.hi) (device); range i goes to d_dst[i] (device)
-static int li_extract(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix, const li_plan &pl, const u8 *in,
+// One run of consecutive spans p0..p1 of an extract wave: the stream's bytes [src_lo, src_hi) are at byte dst
+// of the wave's input
+struct li_run_in { u32 p0, p1; u64 src_lo, src_hi, dst; };
+
+// Range i goes to d_dst[i] (device).  The input: d_in holds the stream's bytes [pl.lo, pl.hi) (device), or, with
+// d_in NULL, h_in is the whole stream (host) and each wave stages only its runs of spans, packed, into
+// ctx->d_stage_in.  Host windows go to the device through ctx->h_win, one copy per wave.
+static int li_extract(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix, const li_plan &pl, const u8 *d_in, const u8 *h_in,
 		      const uint64_t *offsets, const size_t *lens, void *const *d_dst, int32_t *results, size_t n)
 {
 	const size_t np = ix->bit.size();
+	const u64 data_end = ix->actual_in - ldb_trl_bytes(ix->format);
 	std::vector<u8> ok(np, 0);		// needed spans that decoded and checked
 	int rc;
 	if (!pl.spans.empty()) {
-		// the split list: the points after the first needed one, rebased to 'in'
 		const u32 p0 = pl.spans.front();
-		std::vector<u64> split;
-		for (size_t q = p0 + 1; q < np; q++) split.push_back(ix->bit[q] - 8 * pl.lo);
-		rc = ldb_reserve_dev(ctx->li_scan, split.size() * 8 + 256);
-		if (rc) return rc;
-		if (!split.empty()) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_scan.p, split.data(), split.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-		ldb_seg_args g0 = {};
-		g0.base = in;
-		g0.in_nbytes = pl.hi - pl.lo;
-		g0.split = (const u64 *)ctx->li_scan.p;
-		g0.nsplit = (u32)split.size();
-		g0.any_header = ix->any_header;
 		const u64 budget = token_budget_bytes();
 		std::vector<int> slot_of(np, -1);	// wave-local index of a span of the current wave
 		for (size_t s0 = 0; s0 < pl.spans.size();) {
-			// ---- one wave: spans that fit the token budget and the staging bound ----
-			std::vector<li_seg_desc> segs;
+			// ---- one wave: spans that fit the token budget and the staging bounds ----
 			std::vector<u32> wp;		// the wave's spans
 			std::vector<u64> soff;		// their staging offsets
-			u64 tok_bytes = 0, stage_bytes = 0;
+			std::vector<li_seg_desc> segs;
+			u64 tok_bytes = 0, stage_bytes = 0, in_bytes = 0;
 			size_t s1 = s0;
 			for (; s1 < pl.spans.size(); s1++) {
 				const u32 p = pl.spans[s1];
@@ -2346,28 +2388,87 @@ static int li_extract(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix,
 				const u32 pfx = p ? LDB_SEG_PREFIX : 0;
 				if (len > 0xfffffff0u - LDB_SEG_PREFIX || ib > 0xfffffff0u) continue;	// past the decoder's limits: BAD_DATA
 				li_seg_desc d;
-				d.start = ix->bit[p] - 8 * pl.lo;
 				d.pfx = pfx;
-				d.split_i = p - p0;	// the index of point p + 1 in the split list
 				d.room = len;
 				d.slot = align_up(pfx + ldb_inflate_tok_cap(ib, len) + 64, 16);
-				const u64 sb = align_up(pfx + len + 16, 16);
-				if (!segs.empty() && (tok_bytes + d.slot > budget || stage_bytes + sb > LI_STAGE_MAX)) break;
+				const u64 sb = align_up(pfx + len + 16, 16), ibs = h_in ? ib + LIBDEFLATE_B200_INDEX_READ_MARGIN + 16 : 0;
+				if (!segs.empty() && (tok_bytes + d.slot > budget || stage_bytes + sb > LI_STAGE_MAX || in_bytes + ibs > LI_STAGE_MAX)) break;
 				segs.push_back(d);
 				wp.push_back(p);
 				soff.push_back(stage_bytes);
 				tok_bytes += d.slot;
 				stage_bytes += sb;
+				in_bytes += ibs;
 			}
 			s0 = s1;
 			const size_t w = segs.size();
 			if (!w) continue;
+			// ---- the wave's input: the device input as it is, or the wave's runs of spans staged ----
+			std::vector<li_run_in> runs;
+			std::vector<size_t> run_of(w);
+			if (!h_in) runs.push_back({p0, (u32)np - 1, pl.lo, pl.hi, 0});
+			for (size_t i = 0; i < w; i++) {
+				if (h_in && (runs.empty() || runs.back().p1 + 1 != wp[i])) runs.push_back({wp[i], wp[i], ix->bit[wp[i]] >> 3, 0, 0});
+				if (h_in) runs.back().p1 = wp[i];
+				run_of[i] = runs.size() - 1;
+			}
+			const u8 *in = d_in;
+			u64 in_n = pl.hi - pl.lo;
+			if (h_in) {
+				in_n = 0;
+				for (li_run_in &r : runs) {
+					r.src_hi = std::min(data_end, ((span_end_bit(ix, r.p1) + 7) >> 3) + LIBDEFLATE_B200_INDEX_READ_MARGIN);
+					r.dst = align_up(in_n, 16);
+					in_n = r.dst + (r.src_hi - r.src_lo);
+				}
+				rc = ldb_reserve_dev(ctx->d_stage_in, in_n + 64);
+				if (rc) return rc;
+				in = (const u8 *)ctx->d_stage_in.p;
+				for (const li_run_in &r : runs)
+					LDB_CUDA_CHECK_RET(cudaMemcpyAsync((u8 *)in + r.dst, h_in + r.src_lo, r.src_hi - r.src_lo, cudaMemcpyHostToDevice, ctx->stream));
+			}
+			// the split list: the points after each run's first span, through the one after its last, rebased
+			std::vector<u64> split;
+			std::vector<u32> split_base(runs.size());
+			for (size_t r = 0; r < runs.size(); r++) {
+				split_base[r] = (u32)split.size();
+				for (size_t q = runs[r].p0 + 1; q <= runs[r].p1 + 1 && q < np; q++) split.push_back(ix->bit[q] - 8 * runs[r].src_lo + 8 * runs[r].dst);
+			}
+			for (size_t i = 0; i < w; i++) {
+				const li_run_in &r = runs[run_of[i]];
+				segs[i].start = ix->bit[wp[i]] - 8 * r.src_lo + 8 * r.dst;
+				segs[i].split_i = split_base[run_of[i]] + (wp[i] - r.p0);	// the index of point p + 1 in the split list
+			}
+			rc = ldb_reserve_dev(ctx->li_scan, split.size() * 8 + 256);
+			if (rc) return rc;
+			if (!split.empty()) LDB_CUDA_CHECK_RET(cudaMemcpyAsync(ctx->li_scan.p, split.data(), split.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+			ldb_seg_args g0 = {};
+			g0.base = in;
+			g0.in_nbytes = in_n;
+			g0.split = (const u64 *)ctx->li_scan.p;
+			g0.nsplit = (u32)split.size();
+			g0.any_header = ix->any_header;
+			// host windows: the wave's, through pinned memory, after the staged spans
+			std::vector<size_t> wslot(w, 0);
+			size_t nwin = 0;
+			for (size_t i = 0; i < w; i++)
+				if (ix->host_win && wp[i]) wslot[i] = nwin++;
+			const u64 o_win = align_up(stage_bytes, 256);
 			const size_t lay = li_layout_bytes(w), rlay = li_resolve_bytes(w);
 			rc = ldb_reserve_dev(ctx->token_scratch, tok_bytes + 256);
 			if (!rc) rc = ldb_reserve_dev(ctx->li_arr, 2 * lay + 2 * rlay + 256);
-			if (!rc) rc = ldb_reserve_dev(ctx->li_planes, stage_bytes + 256);
+			if (!rc) rc = ldb_reserve_dev(ctx->li_planes, o_win + nwin * (size_t)LDB_SEG_PREFIX + 256);
+			if (!rc && nwin) rc = ldb_reserve_pinned(ctx->h_win, nwin * (size_t)LDB_SEG_PREFIX);
 			if (rc) return rc;
 			u8 *arr = (u8 *)ctx->li_arr.p, *stage = (u8 *)ctx->li_planes.p;
+			if (nwin) {
+				for (size_t i = 0; i < w; i++)
+					if (wp[i]) memcpy((u8 *)ctx->h_win.p + wslot[i] * (size_t)LDB_SEG_PREFIX, ix->h_win.data() + (size_t)(wp[i] - 1) * LDB_SEG_PREFIX, LDB_SEG_PREFIX);
+				LDB_CUDA_CHECK_RET(cudaMemcpyAsync(stage + o_win, ctx->h_win.p, nwin * (size_t)LDB_SEG_PREFIX, cudaMemcpyHostToDevice, ctx->stream));
+			}
+			auto win_of = [&](size_t i) -> const u8 * {
+				return ix->host_win ? stage + o_win + wslot[i] * (size_t)LDB_SEG_PREFIX : ix->d_win + (size_t)(wp[i] - 1) * LDB_SEG_PREFIX;
+			};
 			// ---- 1. decode every span at once (RAW, from its point to the next) ----
 			ldb_inflate_args a;
 			ldb_seg_info *d_info;
@@ -2383,7 +2484,8 @@ static int li_extract(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix,
 				const ldb_seg_info &r = info[i];
 				const u32 p = wp[i];
 				const bool last = p + 1 == np;
-				const bool stop = last ? r.verdict == LDB_SUCCESS && r.end + pl.lo == ix->actual_in - ldb_trl_bytes(ix->format)
+				const li_run_in &ri = runs[run_of[i]];
+				const bool stop = last ? r.verdict == LDB_SUCCESS && r.end + ri.src_lo - ri.dst == data_end
 						       : r.verdict == LDB_SEG_STOPPED && r.split_j == segs[i].split_i;
 				good[i] = stop && r.out_len == segs[i].room && r.reach <= segs[i].pfx;
 			}
@@ -2416,7 +2518,7 @@ static int li_extract(libdeflate_b200_ctx *ctx, const libdeflate_b200_index *ix,
 				for (size_t j = 0; j < gs.size(); j++) {
 					const size_t i = grp ? redo[j] : j;
 					if (good[i] && (grp || !info[i].overflow) && wp[i])
-						pre.push_back({ix->d_win + (size_t)(wp[i] - 1) * LDB_SEG_PREFIX, tok + off, LDB_SEG_PREFIX});
+						pre.push_back({win_of(i), tok + off, LDB_SEG_PREFIX});
 					off += gs[j].slot;
 				}
 			}
@@ -2496,7 +2598,7 @@ extern "C" int libdeflate_b200_index_extract(struct libdeflate_b200_ctx *ctx, co
 	int rc = li_plan_of(ctx, ix, in_nbytes, h_offsets, h_lens, n_ranges, &pl);
 	if (rc) return rc;
 	if (n_ranges && (!d_dst || !h_results)) return ldb_fail(cudaErrorInvalidValue, "index_extract: no destinations or results", __FILE__, __LINE__);
-	return li_extract(ctx, ix, pl, (const u8 *)d_in + pl.lo, h_offsets, h_lens, d_dst, h_results, n_ranges);
+	return li_extract(ctx, ix, pl, (const u8 *)d_in + pl.lo, nullptr, h_offsets, h_lens, d_dst, h_results, n_ranges);
 }
 
 extern "C" int libdeflate_b200_index_extract_host(struct libdeflate_b200_ctx *ctx, const struct libdeflate_b200_index *ix, const void *in,
@@ -2510,7 +2612,7 @@ extern "C" int libdeflate_b200_index_extract_host(struct libdeflate_b200_ctx *ct
 	if (rc) return rc;
 	if (n_ranges && (!h_dst || !h_results)) return ldb_fail(cudaErrorInvalidValue, "index_extract_host: no destinations or results", __FILE__, __LINE__);
 	stream_quiesce quiesce(ctx);
-	// only the compressed bytes the decode reads, and the ranges at their host alignment phases
+	// the ranges at their host alignment phases (each wave stages the compressed bytes of its own spans)
 	std::vector<size_t> doff(n_ranges);
 	size_t total = 0;
 	for (size_t k = 0; k < n_ranges; k++) {
@@ -2518,14 +2620,12 @@ extern "C" int libdeflate_b200_index_extract_host(struct libdeflate_b200_ctx *ct
 		doff[k] = total;
 		total += h_lens[k];
 	}
-	u8 *d_in, *d_out;
-	rc = stage_one(ctx, ctx->d_stage_in, (const u8 *)in + pl.lo, pl.hi - pl.lo, true, &d_in);
-	if (!rc) rc = ldb_reserve_dev(ctx->d_stage_out, total + 64);
+	rc = ldb_reserve_dev(ctx->d_stage_out, total + 64);
 	if (rc) return rc;
-	d_out = (u8 *)ctx->d_stage_out.p;
+	u8 *d_out = (u8 *)ctx->d_stage_out.p;
 	std::vector<void *> dd(n_ranges);
 	for (size_t k = 0; k < n_ranges; k++) dd[k] = d_out + doff[k];
-	rc = li_extract(ctx, ix, pl, d_in, h_offsets, h_lens, dd.data(), h_results, n_ranges);
+	rc = li_extract(ctx, ix, pl, nullptr, (const u8 *)in, h_offsets, h_lens, dd.data(), h_results, n_ranges);
 	if (rc) return rc;
 	for (size_t k = 0; k < n_ranges; k++)
 		if (h_results[k] == LDB_SUCCESS && h_lens[k])
@@ -2549,6 +2649,10 @@ struct libdeflate_b200_decompress_stream {
 	bool header;		// the wrapper header has been parsed
 	bool ended;		// the final block is delivered: the trailer is next
 	bool finished;
+	bool succeeded;		// finished with SUCCESS
+	u64 in_base;		// input bytes consumed before the bytes held
+	bool indexed;		// made by create_indexed ...
+	li_index_sink *index;	// ... and collecting its index here until take_index (host memory only)
 };
 
 extern "C" struct libdeflate_b200_decompress_stream *
@@ -2578,7 +2682,28 @@ libdeflate_b200_decompress_stream_create(struct libdeflate_b200_ctx *ctx, int fo
 	s->total = 0;
 	s->sum = format == LDB_FMT_ZLIB ? 1 : 0;
 	s->header = format == LDB_FMT_RAW;
-	s->ended = s->finished = false;
+	s->ended = s->finished = s->succeeded = false;
+	s->in_base = 0;
+	s->indexed = false;
+	s->index = nullptr;
+	return s;
+}
+
+extern "C" struct libdeflate_b200_decompress_stream *
+libdeflate_b200_decompress_stream_create_indexed(struct libdeflate_b200_ctx *ctx, int format, size_t spacing)
+{
+	if (spacing > LI_INDEX_SPACING_MAX) {
+		ldb_fail(cudaErrorInvalidValue, "decompress_stream_create_indexed: spacing above 1 GiB", __FILE__, __LINE__);
+		return nullptr;
+	}
+	libdeflate_b200_decompress_stream *s = libdeflate_b200_decompress_stream_create(ctx, format);
+	if (!s) return nullptr;
+	s->indexed = true;
+	s->index = new li_index_sink();
+	s->index->spacing = spacing ? spacing : LIBDEFLATE_B200_INDEX_SPACING;
+	s->index->host = true;
+	s->index->bit.push_back(0);	// (a wrapper's bytes are added once it is parsed)
+	s->index->out.push_back(0);
 	return s;
 }
 
@@ -2589,7 +2714,42 @@ extern "C" void libdeflate_b200_decompress_stream_destroy(struct libdeflate_b200
 	cudaStreamSynchronize(s->ctx->stream);
 	cudaFree(s->d_in);
 	cudaFree(s->d_win);
+	delete s->index;
 	delete s;
+}
+
+extern "C" struct libdeflate_b200_index *libdeflate_b200_decompress_stream_take_index(struct libdeflate_b200_decompress_stream *s)
+{
+	auto bad = [](const char *why) -> libdeflate_b200_index * { ldb_fail(cudaErrorInvalidValue, why, __FILE__, __LINE__); return nullptr; };
+	if (!s) return bad("decompress_stream_take_index: no stream");
+	if (!s->indexed) return bad("decompress_stream_take_index: a plain stream collects no index (decompress_stream_create_indexed)");
+	if (!s->index) return bad("decompress_stream_take_index: the index was taken already");
+	if (!s->succeeded)
+		return bad(s->finished ? "decompress_stream_take_index: the stream ended with BAD_DATA"
+				       : "decompress_stream_take_index: no write has returned SUCCESS yet");
+	li_index_sink *k = s->index;
+	k->crc.push_back(k->span_crc);
+	// (a point at the stream's end, before an empty final block, has an empty span: it is no point)
+	while (k->out.size() > 1 && k->out.back() == s->total) {
+		k->bit.pop_back();
+		k->out.pop_back();
+		k->crc.pop_back();
+		k->h_win.resize(k->h_win.size() - LDB_SEG_PREFIX);
+	}
+	libdeflate_b200_index *ix = index_new(s->ctx);
+	ix->format = s->format;
+	ix->any_header = k->block_start;
+	ix->in_nbytes = ix->actual_in = s->in_base;
+	ix->out_nbytes = s->total;
+	ix->spacing = k->spacing;
+	ix->bit.swap(k->bit);
+	ix->out.swap(k->out);
+	ix->crc.swap(k->crc);
+	ix->host_win = true;
+	ix->h_win.swap(k->h_win);
+	delete k;
+	s->index = nullptr;
+	return ix;
 }
 
 extern "C" size_t libdeflate_b200_decompress_stream_pending(const struct libdeflate_b200_decompress_stream *s)
@@ -2633,13 +2793,35 @@ static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t
 	bool header = s->header, ended = s->ended;
 	u64 total = s->total;
 	u32 sum = s->sum;
+	// (an indexed stream's points, windows and span CRCs of this write are dropped again unless it commits)
+	struct sink_undo {
+		li_index_sink *k;
+		size_t np, nwin, ncrc;
+		u32 span_crc;
+		bool block_start;
+		~sink_undo()
+		{
+			if (!k) return;
+			k->bit.resize(np);
+			k->out.resize(np);
+			k->h_win.resize(nwin);
+			k->crc.resize(ncrc);
+			k->span_crc = span_crc;
+			k->block_start = block_start;
+		}
+	} undo = {s->index, 0, 0, 0, 0, false};
+	if (s->index) undo = {s->index, s->index->out.size(), s->index->h_win.size(), s->index->crc.size(), s->index->span_crc, s->index->block_start};
 	// ---- the wrapper header, parsed on the host from the first bytes (more of them until it is complete) ----
 	if (!header) {
 		long hb;
 		int rc = wrapper_bytes(ctx, held, have, s->format, &hb);
 		if (rc) return rc;
 		if (hb == -1) r = LDB_BAD_DATA;
-		else if (hb >= 0) { header = true; used = (size_t)hb; }
+		else if (hb >= 0) {
+			header = true;
+			used = (size_t)hb;
+			if (s->index) s->index->bit[0] = 8 * (s->in_base + used);	// point 0: the first DEFLATE bit
+		}
 	}
 	// ---- the complete blocks that fit, from the first undelivered one -------------------------------
 	const u32 trl = ldb_trl_bytes(s->format);
@@ -2657,6 +2839,11 @@ static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t
 		call.mode = LDB_SEG_STREAM | (last ? 0u : LDB_SEG_OPEN);
 		call.out = (u8 *)d_out;
 		call.room = out_avail;
+		call.index = s->index;
+		if (s->index) {
+			s->index->out0 = total;
+			s->index->bit0 = 8 * (s->in_base + used);
+		}
 		li_run run;
 		int rc = li_chain(ctx, call, &run);
 		if (rc) return rc;
@@ -2674,6 +2861,26 @@ static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t
 		xp[0] = 0x00800000u;	// x^8
 		for (int i = 1; i < 64; i++) xp[i] = ldb_mulmodp(xp[i - 1], xp[i - 1]);
 		for (size_t i = 0; i < nch; i++) sum = ldb_sum_combine(s->format, xp, sum, sums[i], run.chain[i].len);
+		if (s->index) {		// the CRC-32 of every chain segment, folded into the spans of the points
+			li_index_sink &k = *s->index;
+			const size_t nc = run.chain.size();
+			std::vector<u32> crcs(sums);
+			if (s->format != LDB_FMT_GZIP) {
+				rc = li_chain_sums(ctx, LDB_FMT_GZIP, (const u8 *)d_out, run.chain, nc, &d_sums, &d_lens);
+				if (rc) return rc;
+				crcs.resize(nc);
+				rc = read_back(ctx, crcs.data(), d_sums, nc * 4);
+				if (rc) return rc;
+			}
+			for (size_t i = 0, q = undo.np; i < nc; i++) {
+				if (q < k.out.size() && k.out[q] == total + run.chain[i].G) {	// a point: its span starts here
+					k.crc.push_back(k.span_crc);
+					k.span_crc = 0;
+					q++;
+				}
+				k.span_crc = ldb_sum_combine(LDB_FMT_GZIP, xp, k.span_crc, crcs[i], run.chain[i].len);
+			}
+		}
 		out_n = run.out;
 		total += run.out;
 		const s32 v = run.v.result;
@@ -2711,6 +2918,8 @@ static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t
 	}
 	if (last && r == LIBDEFLATE_B200_MORE_INPUT) r = LDB_BAD_DATA;	// every complete block is delivered, the stream has not ended
 	// ---- commit -------------------------------------------------------------------------------------------
+	undo.k = nullptr;
+	s->in_base += used;
 	s->off += used;
 	s->pend = have - used;
 	s->bit = bit;
@@ -2719,6 +2928,7 @@ static int ds_write(libdeflate_b200_decompress_stream *s, const void *in, size_t
 	s->total = total;
 	s->sum = sum;
 	s->finished = r == LDB_SUCCESS || r == LDB_BAD_DATA;
+	s->succeeded = r == LDB_SUCCESS;
 	if (s->finished) s->pend = 0;
 	*out_nbytes = out_n;
 	if (out_needed) *out_needed = r == LIBDEFLATE_B200_MORE_OUTPUT ? need : 0;
